@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- SiamMOT hot-path throughput on B200 (contract: see the task statement / DESIGN.md).
+"""bench.py -- SiamMOT hot-path throughput on one or more H100 GPUs (see DESIGN.md).
 
 A "step" is one frame through the per-frame hot path (backbone -> FPN -> RPN -> box head -> EMM with
 30 tracks in memory -> refinement -> solver -> next-frame memory) on the BASELINE.json configs[1]
@@ -9,7 +9,7 @@ rule (image_augmentation.py:21-42), DLA-34-FPN + EMM, fp16 storage / fp32 accumu
 pinned host memory (per frame: H2D, test transform on the device, hot path, packed result D2H -- all inside the wall-clock
 region); `e2e.per_frame_call`: the same frames through model(frame), one blocking call per frame.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--dtype float16|float32]
+  python bench.py [--gpus N] [--steps K] [--regions R] [--warmup W] [--dtype float16|float32] [--dump-outputs DIR]
   python bench.py --impl reference ...     # the reference path on the host CPU (oracle port)
   torchrun --nproc-per-node N bench.py --gpus N ...   # one process per GPU, independent streams
 
@@ -32,7 +32,7 @@ import torch  # noqa: E402
 H_NET, W_NET = 704, 1280      # 1280x720 after the reference's test-time resize (SURVEY.md fact 5)
 H_SRC, W_SRC = 720, 1280      # the decoded video frame (RGB uint8)
 N_TRACKS = 30
-N_FRAMES = 32                 # distinct frames resident in HBM: 32 x 10.8 MB = 346 MB > 126 MB L2
+N_FRAMES = 32                 # distinct frames resident in HBM: 32 x 10.8 MB = 346 MB > the 50 MB L2 of an H100
 METRIC = "tracker FPS @720p (DLA34-FPN+EMM, 30 tracks)"
 WORKLOAD = "720p synthetic clip -> 3x704x1280, DLA-34-FPN + EMM, 30 active tracks, 1 frame per step"
 CFG_OVERRIDES = []
@@ -67,10 +67,10 @@ def select_workload(name):
 
 
 def config_dict(world=1):
-    """The `config` object of the JSON line: identical for both arms (ours / --impl reference), so the driver compares like with
+    """The `config` object of the JSON line: identical for both arms (ours / --impl reference), so two runs compare like with
     like.  Arm-specific notes (API used, graphs, baseline note) live in `notes`, outside it."""
     return {"workload": WORKLOAD, "net_input": [3, H_NET, W_NET], "source_frame": [H_SRC, W_SRC, 3], "frames_resident": N_FRAMES,
-            "l2": "inputs (%d MB of frames + activations) exceed the 126 MB L2" % (N_FRAMES * 3 * H_NET * W_NET * 4 // 1000000),
+            "l2": "inputs (%d MB of frames + activations) exceed the 50 MB L2 of an H100" % (N_FRAMES * 3 * H_NET * W_NET * 4 // 1000000),
             "tracks_in_memory": N_TRACKS, "parallelism": "1 stream per GPU x %d" % world}
 
 
@@ -186,7 +186,7 @@ def make_frames_u8(n, cfg):
 
 
 # --------------------------------------------------------------------------------------------------
-# clocks sampling (B200_PROFILING.md recipe)
+# clocks sampling
 # --------------------------------------------------------------------------------------------------
 class ClockSampler(object):
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
@@ -294,13 +294,27 @@ def kernels_per_frame(h):
     return n
 
 
-REPEATS = 5   # least number of timed regions per arm: the line reports the median region
+def region_sizes(steps, regions):
+    """The K timed steps of an arm as `regions` consecutive regions (sizes differ by at most one): every arm times exactly K
+    steps, and `spread` shows the rate of each region."""
+    r = max(1, min(int(regions), int(steps)))
+    return [steps // r + (1 if i < steps % r else 0) for i in range(r)]
 
 
-def repeats(steps):
-    """Timed regions per arm: at least REPEATS, and enough short ones to cover ~0.4 s (a 20-step region is 16 ms: one scheduler
-    hiccup on a shared host is 10 % of it, and 5 such regions do not make a stable median; 20 do and still cost < 1 s)."""
-    return REPEATS if REPEATS < 5 else max(REPEATS, min(25, -(-400 // max(int(steps), 1))))
+def dump_outputs(out_dir, res):
+    """What the timed path returned for its last step, as its caller receives it (a BoxList: the boxes and every field; the
+    reference arm: the oracle's dict of tensors), one .npy per array: floating arrays as float32, integer ones (ids, labels)
+    as float64 so that they stay exact."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    if isinstance(res, dict):
+        arrays = {k: v for k, v in res.items() if torch.is_tensor(v)}
+    else:
+        arrays = {"boxes": res.bbox}
+        arrays.update({f: res.get_field(f) for f in res.fields()})
+    for name, t in arrays.items():
+        t = t.detach().cpu()
+        np.save(os.path.join(out_dir, name + ".npy"), t.float().numpy() if t.is_floating_point() else t.double().numpy())
 
 
 def run_ours(args):
@@ -337,9 +351,11 @@ def run_ours(args):
         torch.cuda.synchronize()
 
     # ---- device-resident arm: `value` (clip API: the detection stage of frame t+1 overlaps the host solver of frame t).
-    # No event timers in this arm (they are on only in the per-frame arm below); REPEATS timed regions of exactly K steps.
+    # No event timers in this arm (they are on only in the per-frame arm below); exactly K timed steps, in --regions regions.
     hook = lambda t: h.restore()
-    h.model.forward_clip([frames_dev[i % N_FRAMES] for i in range(max(args.warmup, 4))], before_frame=hook)
+    sizes = region_sizes(args.steps, getattr(args, "regions", 1))
+    # warm-up: at least one untimed clip as long as a timed region, so the timed window meets no shape for the first time
+    h.model.forward_clip([frames_dev[i % N_FRAMES] for i in range(max(args.warmup, 4, sizes[0]))], before_frame=hook)
     seq = [frames_dev[(args.warmup + i) % N_FRAMES] for i in range(args.steps)]
     h.eng.timers = None
     sampler = ClockSampler(local)
@@ -349,18 +365,23 @@ def run_ours(args):
     value_ms = []
     h.eng.host_timers = {}
     t_loop0 = time.perf_counter()
-    for rep in range(repeats(args.steps)):
+    results, done = [], 0
+    for n in sizes:
         barrier()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
-        results = h.model.forward_clip(seq, before_frame=hook)
+        results += h.model.forward_clip(seq[done:done + n], before_frame=hook)
         e1.record()
         barrier()
         value_ms.append(e0.elapsed_time(e1))
+        done += n
+    assert len(results) == args.steps
     host_t, h.eng.host_timers = h.eng.host_timers, None
     ntrk = sum(int((r.get_field("ids") >= 0).sum()) for r in results)
     r = results[-1]
-    ms = median(value_ms)
+    ms = sum(value_ms)
+    if getattr(args, "dump_outputs", None) and rank == 0:
+        dump_outputs(args.dump_outputs, r)
 
     # ---- end-to-end arm through the public API with HOST frames: `e2e`.  The call a user makes per decoded frame:
     # model(uint8 HWC frame) -> H2D of the frame, test transform on the device, the whole hot path, D2H of the result.
@@ -381,22 +402,23 @@ def run_ours(args):
     # clip are on the host, pinned): per frame, the uint8 frame's H2D copy + test transform + detection stage run on the side
     # stream while the previous frame's track stage / host solver run; results arrive as CPU BoxLists (packed block D2H).
     def e2e_clip_loop(src):
-        h.model.forward_clip([src[i % N_FRAMES] for i in range(max(args.warmup, 4))], before_frame=hook)
+        h.model.forward_clip([src[i % N_FRAMES] for i in range(max(args.warmup, 4, sizes[0]))], before_frame=hook)
         seq_h = [src[(args.warmup + i) % N_FRAMES] for i in range(args.steps)]
-        dts = []
-        for rep in range(repeats(args.steps)):
+        dts, res, done = [], [], 0
+        for n in sizes:
             barrier()
             t0 = time.perf_counter()
-            res = h.model.forward_clip(seq_h, before_frame=hook)
+            res += h.model.forward_clip(seq_h[done:done + n], before_frame=hook)
             torch.cuda.synchronize()
             dts.append(time.perf_counter() - t0)
-            assert len(res) == args.steps and all(r.bbox.device.type == "cpu" for r in res)
+            done += n
+        assert len(res) == args.steps and all(r.bbox.device.type == "cpu" for r in res)
         return dts, sum(int((r.get_field("ids") >= 0).sum()) for r in res)
 
     e2e_clip_s, e2e_clip_err, e2e_clip_all = None, None, []
     try:
         e2e_clip_all, ntrk_clip = e2e_clip_loop(frames_u8)
-        e2e_clip_s = median(e2e_clip_all)
+        e2e_clip_s = sum(e2e_clip_all)
         if ntrk_clip != ntrk:   # same frames, same restored memory: the from-host clip must track exactly what `value` tracked
             e2e_clip_err = "clip-from-host tracked %d boxes, device-resident clip %d" % (ntrk_clip, ntrk)
     except Exception as exc:   # keep the per-frame number as the headline rather than lose the line
@@ -453,7 +475,7 @@ def run_ours(args):
         peaks = json.load(open(os.path.join(REPO, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
+    hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
     esz = 2 if args.dtype == "float16" else 4
     S_, T_ = h.eng.s_res, h.eng.t_res
     xc_bytes = N_TRACKS * h.eng.C * (S_ * S_ + T_ * T_ + (S_ - T_ + 1) ** 2) * esz      # SURVEY.md 8(d): N*C*1381*b at S=30, T=15
@@ -484,10 +506,11 @@ def run_ours(args):
                          "e2e.per_frame_call: model(frame) once per frame; "
                          "model.results_on_host = True (CPU BoxLists from the packed result block the engine copies D2H)",
                   "baseline_note": "17 FPS = README.md:22 'a single modern GPU', unnamed hardware",
-                  "repeats": "%d timed regions of exactly %d steps per arm; value / e2e are the median region (max over ranks)" % (repeats(args.steps), args.steps),
+                  "regions": "exactly %d timed steps per arm, in %d consecutive regions of %s steps; value / e2e = steps / total time "
+                             "(max over ranks)" % (args.steps, len(sizes), sizes),
                   "numa_cpus_bound": numa_cpus},
-        "spread": {"value_fps": [round(world * args.steps / (x * 1e-3), 1) for x in value_ms],
-                   "e2e_fps": [round(world * args.steps / x, 1) for x in e2e_clip_all],
+        "spread": {"value_fps": [round(world * n / (x * 1e-3), 1) for n, x in zip(sizes, value_ms)],
+                   "e2e_fps": [round(world * n / x, 1) for n, x in zip(sizes, e2e_clip_all)],
                    "note": "this rank's regions; e2e may exceed value by a few per cent: the device-resident arm reads 10.8 MB fp32 "
                            "frames from HBM (image_to_nhwc), the host arm uploads 2.8 MB uint8 frames and resamples on the side stream"},
         "e2e": {"value": round(e2e_fps, 2), "unit": "frames/s",
@@ -511,7 +534,7 @@ def run_ours(args):
                      "timing": "10 CUDA-event brackets (after 3 warm-up ones) of 20 back-to-back launches of the frame's own correlation "
                                "call on its buffers, right after the timed region; `us_per_launch` is the CUDA-graph replay of the 20 "
                                "launches (the product issues the track stage as a graph), `us_per_launch_eager` the ctypes launch loop",
-                     "peak_source": "MEASURED_PEAKS.json (burst copy)" if peaks else "fallback 6650 GB/s",
+                     "peak_source": "MEASURED_PEAKS.json (burst copy)" if peaks else "fallback 3350 GB/s (H100 SXM data sheet)",
                      "flops_per_launch": N_TRACKS * h.eng.C * 2 * (S_ - T_ + 1) ** 2 * T_ * T_,
                      "note": getattr(tp, "xcorr_note", "")},
         "stage_ms": {"static_graph": round(static_ms, 4), "preprocess_incl_h2d": round(prep_ms, 4),
@@ -632,7 +655,7 @@ def run_experimental_child(args):
         pass
     esz = 2 if args.dtype == "float16" else 4
     xc_bytes = N_TRACKS * h.eng.C * (30 * 30 + 15 * 15 + 16 * 16) * esz
-    print(json.dumps(experimental_arms(h, args, frames_dev, frames_u8, hook, None, tp, float(peaks.get("hbm_gbs", 6650.0)), xc_bytes)))
+    print(json.dumps(experimental_arms(h, args, frames_dev, frames_u8, hook, None, tp, float(peaks.get("hbm_gbs", 3350.0)), xc_bytes)))
 
 
 def experimental_arms(h, args, frames_dev, frames_u8, hook, ntrk_ref, tp, hbm_peak, xc_bytes):
@@ -645,7 +668,7 @@ def experimental_arms(h, args, frames_dev, frames_u8, hook, ntrk_ref, tp, hbm_pe
     from siammot_b200._lib import check, stream_ptr
     eng = h.eng
     res = {}
-    steps = min(args.steps, 100)
+    steps = args.steps
     seq = [frames_dev[(args.warmup + i) % N_FRAMES] for i in range(steps)]
     seq_h = [frames_u8[(args.warmup + i) % N_FRAMES] for i in range(steps)]
     ref_trk = None
@@ -823,14 +846,15 @@ def run_reference(args):
     warm = max(args.warmup, 0)
     for i in range(warm):
         step(i)
-    # bounded: at ~1-2 frames/s the whole run must end within a few minutes
-    steps = min(args.steps, 60)
+    steps = args.steps
     ntrk = 0
     t0 = time.perf_counter()
     for i in range(steps):
         out = step(warm + i)
         ntrk += int((out["ids"] >= 0).sum()) if isinstance(out, dict) else int((out.get_field("ids") >= 0).sum())
     dt = time.perf_counter() - t0
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, out)
     fps = steps / dt
     world = int(os.environ.get("WORLD_SIZE", 1)) if (args.gpus > 1 and "RANK" in os.environ) else 1
     cfgd = config_dict(world)
@@ -841,7 +865,7 @@ def run_reference(args):
         "vs_baseline": None, "dtype": "f32", "data": "synthetic",
         "config": cfgd,
         "notes": {"what": "reference algorithm on the host CPU (oracle port, fp32; the reference itself needs maskrcnn_benchmark which "
-                          "is not installable offline); steps capped at 60; rank 0 only, %d torch threads" % cores},
+                          "is not installable offline); rank 0 only, %d torch threads" % cores},
         "cpu_baseline": {"value": round(fps, 4), "unit": "frames/s", "cores": cores, "kind": "port",
                          "sample": "%d full frames (%dx%d, %d tracks) after %d warm-up frames" % (steps, H_NET, W_NET, N_TRACKS, warm)},
         "e2e": {"value": round(fps, 4), "unit": "frames/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}))
@@ -850,11 +874,17 @@ def run_reference(args):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=100)
+    ap.add_argument("--steps", type=int, default=100, help="timed steps (frames) of every arm")
+    ap.add_argument("--regions", type=int, default=1,
+                    help="split the timed steps of the clip arms into this many consecutive timed regions (1..steps); "
+                         "the number of timed steps stays --steps")
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--dtype", default="float16", choices=["float16", "float32"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the result of the last timed step (boxes and every result field) as "
+                         "DIR/<name>.npy; the inputs are seeded, so runs with the same arguments can be compared array by array")
     ap.add_argument("--experimental", default="off", choices=["subprocess", "inproc", "off", "child"],
                     help="information-only A/B arms of the pipeline switches (all of them are measured defaults since round 2, so "
                          "this is off unless asked for): in a child process after the line is final, in this process under a "
@@ -863,6 +893,10 @@ def main():
                     help="720p30 = BASELINE.json configs[1] (the metric's configuration, default); 1080p80 = configs[2]; "
                          "r50_720p30 = configs[4]")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if not 1 <= args.regions <= args.steps:
+        ap.error("--regions must lie in 1..--steps")
     select_workload(args.workload)
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     if args.impl == "reference":

@@ -1,4 +1,4 @@
-/* smot.h -- C ABI of the SiamMOT B200 hot-path library (libsmot.so, sm_100a only).
+/* smot.h -- C ABI of the SiamMOT hot-path library (libsmot.so, sm_90a / H100 only).
  *
  * Drop-in boundary.  The reference (amazon-science/siam-mot) reaches native code on its per-frame
  * inference path in two ways, both replaced here:
@@ -70,7 +70,7 @@ typedef struct {
   int in_dtype;  /* SMOT_F32 | SMOT_F16: dtype of in, weight, residual */
   int out_dtype; /* SMOT_F32 | SMOT_F16 */
   int algo;      /* SMOT_CONV_* */
-  /* optional scratch for split-K (tcgen05 path, few output tiles x long K): fp32 partial tiles, summed in split
+  /* optional scratch for split-K (wgmma path, few output tiles x long K): fp32 partial tiles, summed in split
    * order by a second kernel.  The first SMOT_CONV_WS_COUNTER_BYTES bytes are reserved (never written); calls
    * sharing a workspace must be stream-ordered -- concurrent streams need one workspace each. */
   void* workspace;

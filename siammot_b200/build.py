@@ -1,4 +1,4 @@
-"""Build libsmot.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Build libsmot.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
 Usage: python -m siammot_b200.build   (also called by __graft_entry__.build()).
 """
@@ -10,8 +10,9 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libsmot.so")
+STAMP = OUT + ".flags"   # the compiler, its version and FLAGS that built OUT: a change to any of them forces a rebuild
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC",
          "-fmad=false",  # contraction only where the kernels say fmaf(): coordinate maths stays IEEE like the CPU reference
          "--expt-relaxed-constexpr", "-cudart", "shared"]
 
@@ -20,9 +21,20 @@ def sources():
     return sorted(glob.glob(os.path.join(CSRC, "*.cu")))
 
 
+def toolchain_stamp():
+    try:
+        version = subprocess.run([NVCC, "--version"], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True).stdout
+    except OSError as exc:
+        version = "unavailable: %s" % exc
+    return "\n".join([NVCC, version.strip(), " ".join(FLAGS)]) + "\n"
+
+
 def needs_build():
-    if not os.path.exists(OUT):
+    if not os.path.exists(OUT) or not os.path.exists(STAMP):
         return True
+    with open(STAMP) as f:
+        if f.read() != toolchain_stamp():
+            return True
     t = os.path.getmtime(OUT)
     deps = sources() + glob.glob(os.path.join(CSRC, "*.cuh")) + [os.path.join(HERE, "..", "include", "smot.h")]
     return any(os.path.getmtime(d) > t for d in deps)
@@ -51,6 +63,8 @@ def build(force=False, verbose=False):
     if r.returncode != 0:
         raise RuntimeError("link failed:\n%s" % r.stdout)
     os.replace(tmp, OUT)
+    with open(STAMP, "w") as f:
+        f.write(toolchain_stamp())
     return OUT
 
 

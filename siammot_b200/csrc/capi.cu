@@ -1,4 +1,4 @@
-// C-ABI glue: error reporting, conv dispatch (SIMT vs tcgen05).
+// C-ABI glue: error reporting, conv dispatch (SIMT vs wgmma).
 #include <stdarg.h>
 #include <string.h>
 
@@ -34,10 +34,10 @@ int sm_count() {
   static int cached[SMOT_MAX_DEVICES];
   int dev = 0;
   cudaGetDevice(&dev);
-  if (dev < 0 || dev >= SMOT_MAX_DEVICES) return 148;
+  if (dev < 0 || dev >= SMOT_MAX_DEVICES) return 132;
   if (!cached[dev]) {
     int n = 0;
-    cached[dev] = (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0) ? n : 148;
+    cached[dev] = (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0) ? n : 132;
   }
   return cached[dev];
 }
@@ -82,7 +82,7 @@ extern "C" int smot_conv2d(const smot_conv_desc* d, void* stream) {
   int algo = d->algo;
   if (algo == SMOT_CONV_AUTO) algo = conv2d_tc_supported(d) ? SMOT_CONV_TCGEN05 : SMOT_CONV_SIMT;
   if (algo == SMOT_CONV_TCGEN05) {
-    SMOT_CHECK_ARG(conv2d_tc_supported(d), "smot_conv2d: tcgen05 path does not support this descriptor");
+    SMOT_CHECK_ARG(conv2d_tc_supported(d), "smot_conv2d: tensor-core (wgmma) path does not support this descriptor");
     return conv2d_tc(d, st);
   }
   if (d->algo == SMOT_CONV_AUTO && conv2d_hires_supported(d)) return conv2d_hires(d, st);  // DLA stem / levels 0-1

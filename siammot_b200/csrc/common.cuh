@@ -1,4 +1,4 @@
-// Shared helpers for the SiamMOT B200 kernels (sm_100a only).
+// Shared helpers for the SiamMOT kernels (sm_90a, H100).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -53,7 +53,7 @@ constexpr int SMOT_MAX_DEVICES = 64;
 // The detection stage is ~110 short kernels in one CUDA graph; at 5-15 us each, the drain -> launch -> prologue
 // gap between consecutive kernels is a large share of the frame.  Kernels launched through launch_pdl() may begin
 // while their predecessor in the stream is still running: they do everything that does not touch the predecessor's
-// data first (barrier init, TMEM allocation, staging constant weights), then pdl_wait() blocks until the predecessor
+// data first (barrier init, staging constant weights), then pdl_wait() blocks until the predecessor
 // has completed and its writes are visible.  pdl_launch_dependents() at the top lets the NEXT kernel start the same
 // way once every CTA of this grid is running.  Both are no-ops for kernels launched the ordinary way.
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }

@@ -2,7 +2,7 @@
 //   base_layer 7x7 3->16, level0 3x3 16->16, level1 3x3/2 16->32, level2.tree1.conv1 3x3/2 32->64
 //   (dla.py:257-260,278-287,34-38).  They hold ~10 % of the FLOPs but ~35 % of the activation bytes: at
 //   704x1280 each reads or writes 14-29 MB and their GEMM N (16..64) and K (147..288) are far too small
-//   for a 128-wide tcgen05 tile, so the bound is HBM, not the tensor pipe.
+//   for a 128-wide wgmma tile, so the bound is HBM, not the tensor pipe.
 // Design: a CTA stages the input halo of an 8x32 (stride 1) or 4x32 (stride 2) output tile ONCE in
 // shared memory (cp.async, zero-fill outside the image = the conv padding) plus the whole weight,
 // every warp then walks the filter taps with warp-level mma.sync.m16n8k16 (A fragments via ldmatrix

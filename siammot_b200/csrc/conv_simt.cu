@@ -8,7 +8,7 @@
 // (reference: siammot/modelling/backbone/dla.py:43-57,181-189).
 //
 // This kernel is what SMOT_F32 runs end to end (bit-for-bit IEEE fp32 multiply-adds, no tensor
-// cores), and in SMOT_F16 it covers the layers the tcgen05 kernel does not take (Cin % 64 != 0,
+// cores), and in SMOT_F16 it covers the layers the wgmma kernel does not take (Cin % 64 != 0,
 // strided, tiny Cout).
 #include "common.cuh"
 

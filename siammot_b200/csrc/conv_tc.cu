@@ -1,4 +1,4 @@
-// tcgen05 / TMA implicit-GEMM convolution for sm_100a (fp16 operands, fp32 accumulation in TMEM).
+// wgmma / TMA implicit-GEMM convolution for sm_90a (fp16 operands, fp32 accumulation in registers).
 //
 // GEMM view as in conv_simt.cu: M = output pixels, N = Cout, K = taps * Cin.  One CTA produces a
 // 128 (pixels) x BN (channels) output tile; the 128 pixels are a TILE_W x TILE_H patch of one image
@@ -6,14 +6,15 @@
 // tile is ONE 4-D TMA box of the NHWC input at offset (s-pad, r-pad): im2col is never built, and
 // the zero padding of the convolution is TMA's out-of-bounds fill.  K advances over
 // taps x (Cin/64): each step stages a 128x64 A box and a BNx64 weight box (both 128B-swizzled,
-// K-major) in a shared-memory ring fed by one TMA-producer thread; one MMA thread issues
-// 4 x tcgen05.mma (M=128, N=BN, K=16) per step into a TMEM accumulator and releases the ring slot
-// with tcgen05.commit; four epilogue warps read the accumulator with tcgen05.ld, apply
+// K-major) in a shared-memory ring fed by one TMA-producer thread.  Two consumer warpgroups own
+// 64 rows of the tile each: per step each issues 4 x wgmma.mma_async (M=64, N=BN, K=16) into its
+// register accumulator and releases the ring slot of the previous step once that step's wgmma
+// group has retired (one group stays in flight).  The same warpgroups then apply
 // scale/bias (+residual) (+ReLU) and store fp16 NHWC with an arbitrary channel pitch (so DLA roots
 // still read their children without a concat).
 //
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM allocator + MMA issuer,
-// warps 2..5 = epilogue (TMEM lane quarter = warp_id % 4).
+// Warp roles (288 threads): warps 0..3 and 4..7 = consumer warpgroups 0 and 1 (tile rows 0..63 / 64..127; a
+// warpgroup must start at a warp index that is a multiple of 4), warp 8 = TMA producer.
 #include <cuda.h>
 #include <cudaTypedefs.h>
 
@@ -28,7 +29,9 @@ namespace smot {
 
 constexpr int TC_BM = 128;
 constexpr int TC_BK = 64;  // fp16 elements = 128 bytes = one swizzle row
-constexpr int TC_THREADS = 192;
+constexpr int TC_CONSUMERS = 256;
+constexpr int TC_THREADS = TC_CONSUMERS + 32;
+constexpr int TC_PRODUCER_WARP = TC_CONSUMERS / 32;
 
 struct TcArgs {
   const float* scale;
@@ -42,10 +45,10 @@ struct TcArgs {
   // split-K (gridDim.z > 1): fp32 partial tiles [z][tile][128][Cout], summed by splitk_reduce_kernel
   int splits, chunks_per_split, num_tiles;
   int cluster_reduce;   // 1: the `splits` CTAs of a tile are one thread-block cluster and finish the tile themselves (no reduce kernel)
-  // in-CTA K slices (splits == 1, slices > 1): ONE CTA runs all `slices` K ranges of `chunks_per_split` chunks, each into its own
-  // TMEM accumulator (BN columns apart), and sums them in slice order in the epilogue -- the bits of the split-K path without
-  // its partial tiles, its reduce kernel and its 8x CTA count
-  int slices, tmem_cols;
+  // in-CTA K slices (splits == 1, slices > 1): ONE CTA runs all `slices` K ranges of `chunks_per_split` chunks, each into a
+  // fresh register accumulator that is added to a running sum in slice order when the range ends -- the bits of the
+  // split-K path without its partial tiles, its reduce kernel and its 8x CTA count
+  int slices;
   float* partial;
   unsigned long long* dbg;  // developer timing probe (SMOT_TC_DEBUG): 8 timestamps of CTA (0,0,0), else null
 };
@@ -59,6 +62,9 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
   asm volatile(
@@ -70,14 +76,11 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// bounded wait: a mis-programmed pipeline must fail the launch, never hang the GPU
+// bounded wait: a mis-programmed pipeline must fail the launch, never hang the GPU.  No printf here: a function call
+// inside the consumer loop would make ptxas serialize every wgmma of the kernel.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  for (uint32_t spin = 0; !mbar_try_wait(bar, parity); ++spin) {
-    if (spin > (1u << 26)) {
-      printf("smot conv_tc: mbarrier wait timed out (block %d,%d thread %d)\n", blockIdx.x, blockIdx.y, threadIdx.x);
-      __trap();
-    }
-  }
+  for (uint32_t spin = 0; !mbar_try_wait(bar, parity); ++spin)
+    if (spin > (1u << 26)) __trap();
 }
 __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* tm, uint64_t* bar, int c0, int c1, int c2, int c3) {
   asm volatile(
@@ -100,169 +103,170 @@ __device__ __forceinline__ unsigned long long gtimer() {
   do {                                                                                                \
     if (a.dbg && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0) a.dbg[i] = gtimer();          \
   } while (0)
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// SM100 shared-memory matrix descriptor: K-major, 128B swizzle, 8-row atoms 1024 B apart
-__device__ __forceinline__ uint64_t umma_desc_sw128(const void* smem) {
+// SM90 shared-memory matrix descriptor: K-major, 128B swizzle, 8-row groups `sbo_bytes` apart (1024 B = dense atoms)
+__device__ __forceinline__ uint64_t gmma_desc_sw128(const void* smem, uint32_t sbo_bytes = 1024u, uint32_t base_offset = 0u) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_u32(smem) & 0x3FFFF) >> 4);  // start address
-  d |= (uint64_t)0 << 16;                            // leading byte offset (unused: one atom along K)
-  d |= (uint64_t)(1024 >> 4) << 32;                  // stride byte offset
-  d |= (uint64_t)1 << 46;                            // descriptor version (SM100)
-  d |= (uint64_t)2 << 61;                            // layout type: SWIZZLE_128B
+  d |= (uint64_t)1 << 16;                            // leading byte offset (unused: one atom along K)
+  d |= (uint64_t)(sbo_bytes >> 4) << 32;             // stride byte offset
+  d |= (uint64_t)(base_offset & 7u) << 49;           // swizzle phase of the start address
+  d |= (uint64_t)1 << 62;                            // layout type: SWIZZLE_128B
   return d;
 }
-// instruction descriptor, kind::f16: D=f32, A=B=f16, both K-major, N>>3 at bit 17, M>>4 at bit 24
-__device__ __forceinline__ uint32_t umma_idesc_f16(int M, int N) {
-  return (1u << 4) | (0u << 7) | (0u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
+
+// wgmma.mma_async m64nNk16, D(f32, registers) = A(f16, smem) * B(f16, smem) (+ D when accum != 0); both operands K-major
+__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t ad, uint64_t bd, uint32_t accum) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+      "}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(ad), "l"(bd), "r"(accum));
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-  uint32_t r[32];
+__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t ad, uint64_t bd, uint32_t accum) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  // the registers are only valid after wait::ld: tie them to the wait so nothing is scheduled across it
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "+r"(r[8]),
-                 "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]), "+r"(r[16]),
-                 "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]), "+r"(r[22]), "+r"(r[23]), "+r"(r[24]),
-                 "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]), "+r"(r[29]), "+r"(r[30]), "+r"(r[31])
-               :
-               : "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+      "}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(ad), "l"(bd), "r"(accum));
+}
+__device__ __forceinline__ void wgmma_n256(float (&d)[128], uint64_t ad, uint64_t bd, uint32_t accum) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+      "}, %128, %129, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(ad), "l"(bd), "r"(accum));
 }
 
-// ---- epilogue warps 2..5: TMEM -> scale / bias (+residual) (+ReLU) -> fp16 NHWC, or the raw fp32 partial tile when K is split
-template <int BN, bool SLICES_OK>
-__device__ __forceinline__ void tc_epilogue(const TcArgs& a, uint32_t tmem_base, float* s_scale, float* s_bias, uint64_t* tmem_full,
-                                            int img, int h0, int w0, int n0) {
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int q = warp & 3;  // TMEM lane quarter this warp may access
-    const int row = q * 32 + lane;
-    const int oh = h0 + row / a.tile_w, ow = w0 + row % a.tile_w;
-    const bool valid = oh < a.H && ow < a.W;
-    const size_t pix = ((size_t)img * a.H + oh) * a.W + ow;
-    // while the main loop runs: park this N-tile's scale / bias in shared memory (read as float4 broadcasts later)
-    for (int i = threadIdx.x - 64; i < BN; i += 128) {
-      s_scale[i] = a.scale ? __ldg(a.scale + n0 + i) : 1.f;
-      s_bias[i] = a.bias ? __ldg(a.bias + n0 + i) : 0.f;
-    }
-    asm volatile("bar.sync 1, 128;" ::: "memory");
-    auto finish = [&](float* v, int c0) {  // scale / bias / residual / ReLU / fp16 store of 32 channels
-      const int n = n0 + c0;
-      if (a.scale) {
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keep the compiler from moving accumulator reads / writes across a wgmma fence or wait
+template <int R>
+__device__ __forceinline__ void wg_fence_acc(float (&d)[R]) {
 #pragma unroll
-        for (int g = 0; g < 8; ++g) {
-          const float4 sc = *reinterpret_cast<const float4*>(s_scale + c0 + 4 * g);
-          v[4 * g] = __fmul_rn(v[4 * g], sc.x), v[4 * g + 1] = __fmul_rn(v[4 * g + 1], sc.y);
-          v[4 * g + 2] = __fmul_rn(v[4 * g + 2], sc.z), v[4 * g + 3] = __fmul_rn(v[4 * g + 3], sc.w);
-        }
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// one 64-channel K chunk: 4 x K=16 steps, +32 bytes (2 x 16B units) per step inside the swizzle atom
+template <int BN>
+__device__ __forceinline__ void wgmma_chunk(float (&d)[BN / 2], uint64_t ad, uint64_t bd, bool accumulate) {
+#pragma unroll
+  for (int k = 0; k < TC_BK / 16; ++k) {
+    const uint32_t acc = (accumulate || k != 0) ? 1u : 0u;
+    if constexpr (BN == 64) wgmma_n64(d, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), acc);
+    else if constexpr (BN == 128) wgmma_n128(d, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), acc);
+    else wgmma_n256(d, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), acc);
+  }
+}
+
+// consumer threads park this N-tile's scale / bias in shared memory, then meet (named barrier 1, consumers only)
+template <int BN>
+__device__ __forceinline__ void tc_stage_scale_bias(const TcArgs& a, float* s_scale, float* s_bias, int n0) {
+  for (int i = threadIdx.x; i < BN; i += TC_CONSUMERS) {
+    s_scale[i] = a.scale ? __ldg(a.scale + n0 + i) : 1.f;
+    s_bias[i] = a.bias ? __ldg(a.bias + n0 + i) : 0.f;
+  }
+  asm volatile("bar.sync 1, %0;" ::"n"(TC_CONSUMERS) : "memory");
+}
+
+// ---- epilogue of one consumer warpgroup: registers -> scale / bias (+residual) (+ReLU) -> fp16 NHWC, or the raw fp32
+// partial tile when K is split.  wgmma's accumulator layout: thread (warp w, lane l) of the warpgroup holds rows
+// 16w + l/4 and 16w + l/4 + 8 of its 64, columns 8j + 2(l%4) and +1 in d[4j + 2h], d[4j + 2h + 1] (h = row half).
+template <int BN>
+__device__ __forceinline__ void tc_epilogue(const TcArgs& a, const float (&d)[BN / 2], const float* s_scale, const float* s_bias,
+                                            int img, int h0, int w0, int n0) {
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127, warp = t >> 5, lane = t & 31;
+  const int cl = 2 * (lane & 3);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = wg * 64 + warp * 16 + (lane >> 2) + 8 * h;
+    if (a.splits > 1) {
+      // ---- split-K: park the raw fp32 partial tile [split][tile][128][Cout]; splitk_reduce_kernel finishes the layer
+      float* mine = a.partial + (((size_t)blockIdx.z * a.num_tiles + blockIdx.x) * TC_BM + row) * a.Cout + n0 + cl;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) *reinterpret_cast<float2*>(mine + 8 * j) = make_float2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
+      continue;
+    }
+    const int oh = h0 + row / a.tile_w, ow = w0 + row % a.tile_w;
+    if (oh >= a.H || ow >= a.W) continue;
+    const size_t pix = ((size_t)img * a.H + oh) * a.W + ow;
+    const __half* rp = a.res ? a.res + pix * a.res_ld + n0 + cl : nullptr;
+    __half* op = a.out + pix * a.out_ld + n0 + cl;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int c = 8 * j + cl;
+      float v0 = d[4 * j + 2 * h], v1 = d[4 * j + 2 * h + 1];
+      if (a.scale) {
+        const float2 sc = *reinterpret_cast<const float2*>(s_scale + c);
+        v0 = __fmul_rn(v0, sc.x), v1 = __fmul_rn(v1, sc.y);
       }
       if (a.bias) {
-#pragma unroll
-        for (int g = 0; g < 8; ++g) {
-          const float4 bi = *reinterpret_cast<const float4*>(s_bias + c0 + 4 * g);
-          v[4 * g] = __fadd_rn(v[4 * g], bi.x), v[4 * g + 1] = __fadd_rn(v[4 * g + 1], bi.y);
-          v[4 * g + 2] = __fadd_rn(v[4 * g + 2], bi.z), v[4 * g + 3] = __fadd_rn(v[4 * g + 3], bi.w);
-        }
+        const float2 bi = *reinterpret_cast<const float2*>(s_bias + c);
+        v0 = __fadd_rn(v0, bi.x), v1 = __fadd_rn(v1, bi.y);
       }
-      if (a.res) {
-        const uint4* rp = reinterpret_cast<const uint4*>(a.res + pix * a.res_ld + n);
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          uint4 rv = __ldg(rp + g);
-          const __half2* h2 = reinterpret_cast<const __half2*>(&rv);
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            float2 f = __half22float2(h2[e]);
-            v[g * 8 + 2 * e] += f.x;
-            v[g * 8 + 2 * e + 1] += f.y;
-          }
-        }
+      if (rp) {
+        const float2 f = __half22float2(*reinterpret_cast<const __half2*>(rp + 8 * j));
+        v0 += f.x, v1 += f.y;
       }
-      if (a.relu) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-      }
-      uint4* op = reinterpret_cast<uint4*>(a.out + pix * a.out_ld + n);
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        uint4 ov;
-        __half2* h2 = reinterpret_cast<__half2*>(&ov);
-#pragma unroll
-        for (int e = 0; e < 4; ++e) h2[e] = __floats2half2_rn(v[g * 8 + 2 * e], v[g * 8 + 2 * e + 1]);
-        op[g] = ov;
-      }
-    };
-    mbar_wait(tmem_full, 0u);
-    if (warp == 2 && lane == 0) TC_STAMP(3);
-    tc_fence_after();
-    if (SLICES_OK && a.slices > 1) {
-      // the accumulators of the K slices, summed in slice order from 0.f: splitk_reduce_kernel's operations on the same values
-#pragma unroll 1
-      for (int c0 = 0; c0 < BN; c0 += 32) {
-        float acc[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) acc[j] = 0.f;
-#pragma unroll 1
-        for (int z = 0; z < a.slices; ++z) {
-          float v[32];
-          tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(z * BN + c0), v);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) acc[j] += v[j];
-        }
-        if (valid) finish(acc, c0);
-      }
-    } else if (a.splits == 1) {
-#pragma unroll 1
-      for (int c0 = 0; c0 < BN; c0 += 32) {
-        float v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, v);
-        if (valid) finish(v, c0);
-      }
-    } else {
-      // ---- split-K: park the raw fp32 partial tile [split][tile][128][Cout]; splitk_reduce_kernel finishes the layer
-      const int tile_id = (int)blockIdx.x;
-      float* mine = a.partial + (((size_t)blockIdx.z * a.num_tiles + tile_id) * TC_BM + row) * a.Cout + n0;
-#pragma unroll 1
-      for (int c0 = 0; c0 < BN; c0 += 32) {
-        float v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, v);
-#pragma unroll
-        for (int g = 0; g < 8; ++g) reinterpret_cast<float4*>(mine + c0)[g] = make_float4(v[4 * g], v[4 * g + 1], v[4 * g + 2], v[4 * g + 3]);
-      }
+      if (a.relu) v0 = fmaxf(v0, 0.f), v1 = fmaxf(v1, 0.f);
+      *reinterpret_cast<__half2*>(op + 8 * j) = __floats2half2_rn(v0, v1);
     }
   }
+}
 
-// ---- split-K finish inside the cluster (replaces splitk_reduce_kernel: 22 launches, ~6 us each, 10 % of a frame in round 1).
+// ---- split-K finish inside the cluster (developer switch SMOT_TC_CLUSTER, replaces splitk_reduce_kernel).
 // The `splits` CTAs of an output tile are launched as ONE thread-block cluster (1,1,splits): they are co-scheduled by the
 // hardware, so after parking their raw fp32 partial tiles in the L2-resident workspace they can meet at a cluster barrier and
 // each finish 128/splits rows of the tile: sum the partials in split order (deterministic, the same order and the same
 // fp32 operations as splitk_reduce_kernel, so the results are bit-identical to it), scale / bias / residual / ReLU, fp16 store.
-// Per CTA: 128 x BN x 4 B of partials read back from L2 (.cg: written by other SMs), ~1 us, instead of a kernel boundary.
 template <int BN>
 __device__ __forceinline__ void tc_splitk_finish(const TcArgs& a, const float* s_scale, const float* s_bias, int img, int h0, int w0,
                                                  int n0) {
-  // all six warps take part; every thread has FIN_ITEMS float4 positions x up to 8 partials in flight before it sums
-  // (the slice is 128 x BN x 4 B per CTA read back from L2 at ~1 us latency: bytes in flight are what bounds it)
+  // all warps take part; every thread has FIN_ITEMS float4 positions x up to 8 partials in flight before it sums
   constexpr int FIN_ITEMS = 3, MAXS = 8;
   const int tid = (int)threadIdx.x;
   const int rows_per = (TC_BM + a.splits - 1) / a.splits;
@@ -324,10 +328,17 @@ struct TcSmem {
   static constexpr int TOTAL = STAGES * STAGE_BYTES + 1024 /*alignment slack*/ + 256 /*barriers*/ + BN * 8 /*scale, bias*/;
 };
 
+// K slices keep a second register accumulator (the running sum): only the variants whose two accumulators fit carry them
 template <int BN, int STAGES>
-__global__ void __launch_bounds__(TC_THREADS) conv_tc_kernel(const __grid_constant__ CUtensorMap tmA,
-                                                             const __grid_constant__ CUtensorMap tmB, const TcArgs a) {
+constexpr bool tc_has_slices() { return STAGES > 2 && BN <= 128; }
+
+// the 2-stage variants (many short tiles) run 2 CTAs per SM: cap their registers accordingly
+template <int BN, int STAGES>
+__global__ void __launch_bounds__(TC_THREADS, STAGES == 2 ? 2 : 1) conv_tc_kernel(const __grid_constant__ CUtensorMap tmA,
+                                                                                  const __grid_constant__ CUtensorMap tmB,
+                                                                                  const TcArgs a) {
   using S = TcSmem<BN, STAGES>;
+  constexpr bool SLICES = tc_has_slices<BN, STAGES>();
   extern __shared__ uint8_t tc_smem_raw[];
   // 128B-swizzled tiles need 1024B-aligned bases
   uint8_t* smem = tc_smem_raw + ((1024u - (smem_u32(tc_smem_raw) & 1023u)) & 1023u);
@@ -336,8 +347,6 @@ __global__ void __launch_bounds__(TC_THREADS) conv_tc_kernel(const __grid_consta
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * S::STAGE_BYTES);
   uint64_t* full = bars;
   uint64_t* empty = bars + STAGES;
-  uint64_t* tmem_full = bars + 2 * STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 1);
   float* s_scale = reinterpret_cast<float*>(smem + STAGES * S::STAGE_BYTES + 256);  // [BN] scale, then [BN] bias
   float* s_bias = s_scale + BN;
 
@@ -353,33 +362,23 @@ __global__ void __launch_bounds__(TC_THREADS) conv_tc_kernel(const __grid_consta
   const int w0 = tw * a.tile_w, h0 = th * a.tile_h;
   const int n0 = blockIdx.y * BN;
   const int all_chunks = a.taps * a.cin_chunks;
-  const bool sliced = STAGES > 2 && a.slices > 1;                        // all K slices in this CTA, one accumulator each
+  const bool sliced = SLICES && a.slices > 1;                             // all K slices in this CTA, one running sum
   const int it0 = sliced ? 0 : (int)blockIdx.z * a.chunks_per_split;    // this CTA's K range [it0, it0 + total)
   const int total = sliced ? all_chunks : min(a.chunks_per_split, all_chunks - it0);
-  const uint32_t tmem_cols = sliced ? (uint32_t)a.tmem_cols : (uint32_t)BN;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
+      mbar_init(&empty[s], 2);  // one arrival per consumer warpgroup
     }
-    mbar_init(tmem_full, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  if (warp == 1) {  // TMEM allocation (whole warp), BN fp32 columns per accumulator
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(tmem_cols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();  // everything above overlapped the previous kernel; its outputs are read (and buffers rewritten) from here on
   if (threadIdx.x == 0) TC_STAMP(1);
 
-  if (warp == 0) {
+  if (warp == TC_PRODUCER_WARP) {
     if (lane == 0) {  // ===== TMA producer =====
       for (int it = 0; it < total; ++it) {
         const int s = it % STAGES;
@@ -392,31 +391,57 @@ __global__ void __launch_bounds__(TC_THREADS) conv_tc_kernel(const __grid_consta
         tma_load_2d(sB + s * S::B_BYTES, &tmB, &full[s], tap * a.Cin + cc * TC_BK, n0);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {  // ===== MMA issuer =====
-      const uint32_t idesc = umma_idesc_f16(TC_BM, BN);
-      for (int it = 0; it < total; ++it) {
-        const int s = it % STAGES;
-        const uint32_t ph = (uint32_t)(it / STAGES) & 1u;
-        mbar_wait(&full[s], ph);
-        if (it == 0) TC_STAMP(2);
-        tc_fence_after();
-        const uint64_t ad = umma_desc_sw128(sA + s * S::A_BYTES);
-        const uint64_t bd = umma_desc_sw128(sB + s * S::B_BYTES);
-        const int sl = sliced ? it / a.chunks_per_split : 0, itl = it - sl * a.chunks_per_split;   // slice, chunk inside it
-        const uint32_t d_tmem = tmem_base + (uint32_t)(sl * BN);
+  } else {  // ===== consumer warpgroups: wgmma main loop, then the epilogue of their 64 rows =====
+    tc_stage_scale_bias<BN>(a, s_scale, s_bias, n0);
+    const int wg = threadIdx.x >> 7;
+    const bool leader = (threadIdx.x & 127) == 0;
+    float acc[BN / 2];
+    float sum[SLICES ? BN / 2 : 1];
 #pragma unroll
-        for (int k = 0; k < TC_BK / 16; ++k)  // +32 bytes (2 x 16B units) per K=16 step inside the swizzle atom
-          umma_f16(d_tmem, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), idesc, (uint32_t)((itl | k) != 0));
-        umma_commit(&empty[s]);  // slot reusable once these MMAs have read it
-      }
-      umma_commit(tmem_full);    // accumulator(s) complete
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    if constexpr (SLICES) {
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) sum[i] = 0.f;
     }
-  } else {  // ===== epilogue warps 2..5 =====
-    tc_epilogue<BN, (STAGES > 2)>(a, tmem_base, s_scale, s_bias, tmem_full, img, h0, w0, n0);
+    for (int it = 0; it < total; ++it) {
+      const int s = it % STAGES;
+      mbar_wait(&full[s], (uint32_t)(it / STAGES) & 1u);
+      if (it == 0 && threadIdx.x == 0) TC_STAMP(2);
+      const int itl = sliced ? it % a.chunks_per_split : it;   // chunk inside this CTA's (or this slice's) K range
+      const uint64_t ad = gmma_desc_sw128(sA + s * S::A_BYTES + wg * (64 * TC_BK * 2));
+      const uint64_t bd = gmma_desc_sw128(sB + s * S::B_BYTES);
+      wg_fence_acc(acc);
+      wg_fence();
+      wgmma_chunk<BN>(acc, ad, bd, itl != 0);
+      wg_commit();
+      wg_wait<1>();                                     // the previous chunk's wgmma group has read its slot
+      wg_fence_acc(acc);
+      if (it > 0 && leader) mbar_arrive(&empty[(it - 1) % STAGES]);
+      if constexpr (SLICES) {
+        if (sliced && (itl == a.chunks_per_split - 1 || it == total - 1)) {
+          // a K slice is complete: add it to the running sum in slice order from 0.f -- splitk_reduce_kernel's operations
+          wg_wait<0>();
+          wg_fence_acc(acc);
+#pragma unroll
+          for (int i = 0; i < BN / 2; ++i) sum[i] += acc[i];
+        }
+      }
+    }
+    wg_wait<0>();
+    wg_fence_acc(acc);
+    if (threadIdx.x == 0) TC_STAMP(3);
+    if constexpr (SLICES) {
+      if (sliced) {
+        tc_epilogue<BN>(a, sum, s_scale, s_bias, img, h0, w0, n0);
+      } else {
+        tc_epilogue<BN>(a, acc, s_scale, s_bias, img, h0, w0, n0);
+      }
+    } else {
+      tc_epilogue<BN>(a, acc, s_scale, s_bias, img, h0, w0, n0);
+    }
+    if (threadIdx.x == 0) TC_STAMP(4);
   }
-  if (warp == 2 && lane == 0) TC_STAMP(4);
-  if constexpr (STAGES > 2)   // the 2-stage variants run 4 CTAs per SM on full-GPU layers: they never split K, keep their registers low
+  if constexpr (STAGES > 2)   // the 2-stage variants run 2 CTAs per SM on full-GPU layers: they never split K, keep their registers low
   if (a.cluster_reduce) {
     // every CTA of the tile's cluster has parked its partial: publish (gpu scope), meet, finish 128 / splits rows each
     __threadfence();
@@ -425,24 +450,17 @@ __global__ void __launch_bounds__(TC_THREADS) conv_tc_kernel(const __grid_consta
     asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
     tc_splitk_finish<BN>(a, s_scale, s_bias, img, h0, w0, n0);
   }
-  tc_fence_before();
-  __syncthreads();
   if (threadIdx.x == 0) TC_STAMP(5);
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(tmem_cols) : "memory");
-  }
 }
 
 // ---------------------------------------------------------------------------------------------
-// 3x3 / stride 1 with a shared-memory resident input halo.
-// conv_tc_kernel re-reads the A operand once per filter tap: 9 x 16 KB per 64-channel chunk and CTA.  Measured,
-// those layers sit at the L2 -> SM throughput cap (~11.5 TB/s over all SMs, profiles/conv_layers_r01_*.txt), not at
-// the tensor pipe.  Here the (8+2) x (16+2) pixel halo of an 8 x 16 output tile is loaded ONCE per channel chunk
-// (one 4-D TMA box, PW pixels per patch row, 128B-swizzled, zero fill = conv padding) and the nine taps are nine
-// shifted views of it: row m = y*8 + x of tap (r, s) is patch pixel (y + r, x + s), i.e. the UMMA descriptor starts
-// (r*PW + s) * 128 B into the patch and steps PW * 128 B between its 8-row groups.  Only the weights still stream per
-// tap (their own ring).  K order: channel chunk outermost, taps inside.
+// 3x3 / stride 1 with a shared-memory resident input halo (developer switch SMOT_TC_HALO).
+// conv_tc_kernel re-reads the A operand once per filter tap: 9 x 16 KB per 64-channel chunk and CTA.  Here the
+// (8+2) x (16+2) pixel halo of an 8 x 16 output tile is loaded ONCE per channel chunk (one 4-D TMA box, PW pixels per
+// patch row, 128B-swizzled, zero fill = conv padding) and the nine taps are nine shifted views of it: row m = y*8 + x of
+// tap (r, s) is patch pixel (y + r, x + s), i.e. the wgmma descriptor of consumer warpgroup g (rows y = 8g..8g+7) starts
+// ((8g + r)*PW + s) * 128 B into the patch and steps PW * 128 B between its 8-row groups.  Only the weights still stream
+// per tap (their own ring).  K order: channel chunk outermost, taps inside.
 // ---------------------------------------------------------------------------------------------
 constexpr int HALO_TW = 8, HALO_TH = 16, HALO_SA = 2;
 
@@ -453,18 +471,8 @@ struct HaloSmem {
   static constexpr int B_BYTES = BN * TC_BK * 2;
   static constexpr int RING = HALO_SA * A_BYTES + SB * B_BYTES;
   static constexpr int TOTAL = RING + 1024 /*alignment slack*/ + 256 /*barriers*/ + BN * 8 /*scale, bias*/;
-  static_assert((2 * HALO_SA + 2 * SB + 2) * 8 <= 256, "barrier block");
+  static_assert((2 * HALO_SA + 2 * SB) * 8 <= 256, "barrier block");
 };
-
-__device__ __forceinline__ uint64_t umma_desc_sw128_rows(const void* smem, uint32_t sbo_bytes, uint32_t base_offset) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_u32(smem) & 0x3FFFF) >> 4);
-  d |= (uint64_t)(sbo_bytes >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)(base_offset & 7u) << 49;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
 
 template <int BN, int PW, int SB>
 __global__ void __launch_bounds__(TC_THREADS) conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA,
@@ -480,8 +488,6 @@ __global__ void __launch_bounds__(TC_THREADS) conv3x3_halo_kernel(const __grid_c
   uint64_t* emptyA = fullA + HALO_SA;
   uint64_t* fullB = emptyA + HALO_SA;
   uint64_t* emptyB = fullB + SB;
-  uint64_t* tmem_full = emptyB + SB;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full + 1);
   float* s_scale = reinterpret_cast<float*>(smem + S::RING + 256);
   float* s_bias = s_scale + BN;
 
@@ -498,26 +504,17 @@ __global__ void __launch_bounds__(TC_THREADS) conv3x3_halo_kernel(const __grid_c
   const int ncc = min(a.chunks_per_split, a.cin_chunks - cc0);
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < HALO_SA; ++i) mbar_init(&fullA[i], 1), mbar_init(&emptyA[i], 1);
-    for (int i = 0; i < SB; ++i) mbar_init(&fullB[i], 1), mbar_init(&emptyB[i], 1);
-    mbar_init(tmem_full, 1);
+    for (int i = 0; i < HALO_SA; ++i) mbar_init(&fullA[i], 1), mbar_init(&emptyA[i], 2);
+    for (int i = 0; i < SB; ++i) mbar_init(&fullB[i], 1), mbar_init(&emptyB[i], 2);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"((uint32_t)BN)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();
 
   // developer probes (timing only, results are garbage): 256 = no MMAs, 512 = no weight loads, 1024 = no patch loads
   const bool no_mma = bo_mode & 256, no_b = bo_mode & 512, no_a = bo_mode & 1024;
-  if (warp == 0) {
+  if (warp == TC_PRODUCER_WARP) {
     if (lane == 0) {  // ===== TMA producer: one halo patch per channel chunk, one weight tile per tap =====
       int ib = 0;
       for (int ic = 0; ic < ncc; ++ic) {
@@ -535,41 +532,42 @@ __global__ void __launch_bounds__(TC_THREADS) conv3x3_halo_kernel(const __grid_c
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {  // ===== MMA issuer =====
-      const uint32_t idesc = umma_idesc_f16(TC_BM, BN);
-      int ib = 0;
-      for (int ic = 0; ic < ncc; ++ic) {
-        const int sa = ic % HALO_SA;
-        if (!no_a) mbar_wait(&fullA[sa], (uint32_t)(ic / HALO_SA) & 1u);
-        const uint8_t* patch = sA + sa * S::A_BYTES;
-        for (int tap = 0; tap < 9; ++tap, ++ib) {
-          const int sb = ib % SB;
-          if (!no_b) mbar_wait(&fullB[sb], (uint32_t)(ib / SB) & 1u);
-          tc_fence_after();
-          const int r = tap / 3, sx = tap - 3 * r;
-          const uint32_t first_row = (uint32_t)(r * PW + sx);   // patch pixel of output row 0 for this tap
-          const uint64_t ad = umma_desc_sw128_rows(patch + first_row * 128u, (uint32_t)PW * 128u, (bo_mode & 1) ? first_row : 0u);
-          const uint64_t bd = umma_desc_sw128(sB + sb * S::B_BYTES);
-          if (!no_mma) {
+  } else {  // ===== consumer warpgroups =====
+    tc_stage_scale_bias<BN>(a, s_scale, s_bias, n0);
+    const int wg = threadIdx.x >> 7;
+    const bool leader = (threadIdx.x & 127) == 0;
+    float acc[BN / 2];
 #pragma unroll
-            for (int k = 0; k < TC_BK / 16; ++k)
-              umma_f16(tmem_base, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), idesc, (uint32_t)((ic | tap | k) != 0));
-          }
-          if (!no_b) umma_commit(&emptyB[sb]);
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int ib = 0;
+    for (int ic = 0; ic < ncc; ++ic) {
+      const int sa = ic % HALO_SA;
+      if (!no_a) mbar_wait(&fullA[sa], (uint32_t)(ic / HALO_SA) & 1u);
+      const uint8_t* patch = sA + sa * S::A_BYTES;
+      for (int tap = 0; tap < 9; ++tap, ++ib) {
+        const int sb = ib % SB;
+        if (!no_b) mbar_wait(&fullB[sb], (uint32_t)(ib / SB) & 1u);
+        const int r = tap / 3, sx = tap - 3 * r;
+        const uint32_t first_row = (uint32_t)((8 * wg + r) * PW + sx);   // patch pixel of this warpgroup's row 0 for this tap
+        const uint64_t ad = gmma_desc_sw128(patch + first_row * 128u, (uint32_t)PW * 128u, (bo_mode & 1) ? first_row : 0u);
+        const uint64_t bd = gmma_desc_sw128(sB + sb * S::B_BYTES);
+        if (!no_mma) {
+          wg_fence_acc(acc);
+          wg_fence();
+          wgmma_chunk<BN>(acc, ad, bd, (ic | tap) != 0);
+          wg_commit();
+          wg_wait<1>();                                   // the previous tap's wgmma group is done with its slots
+          wg_fence_acc(acc);
         }
-        if (!no_a) umma_commit(&emptyA[sa]);   // all nine taps of this patch have been read
+        if (ib > 0 && leader) {
+          if (!no_b) mbar_arrive(&emptyB[(ib - 1) % SB]);
+          if (tap == 0 && !no_a) mbar_arrive(&emptyA[(ic - 1) % HALO_SA]);   // all nine taps of the previous patch are read
+        }
       }
-      umma_commit(tmem_full);
     }
-  } else {
-    tc_epilogue<BN, false>(a, tmem_base, s_scale, s_bias, tmem_full, img, h0, w0, n0);
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)BN) : "memory");
+    wg_wait<0>();
+    wg_fence_acc(acc);
+    tc_epilogue<BN>(a, acc, s_scale, s_bias, img, h0, w0, n0);
   }
 }
 
@@ -617,6 +615,10 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(const TcArgs a) {
 
 // ---- host side ------------------------------------------------------------------------------
 constexpr int SMOT_TC_DEFAULT_MAXSPLIT = 8;
+// The split factor of a layer fixes the order in which its fp32 partial sums are added, so it is a function of the layer
+// alone and not of the device it runs on: the same weights and frames give the same bits on any GPU.  The basis is a
+// CTA budget of 148 (a little more than the 132 SMs of an H100: the split CTAs of few-tile layers fill one wave either way).
+constexpr int SMOT_TC_SPLIT_BASIS = 148;
 static PFN_cuTensorMapEncodeTiled get_encode() {
   static PFN_cuTensorMapEncodeTiled fn = nullptr;
   static bool tried = false;
@@ -634,7 +636,7 @@ static bool encode_map(CUtensorMap* tm, const void* base, int rank, const uint64
                        const uint32_t* box, const uint32_t* estr_in = nullptr) {
   PFN_cuTensorMapEncodeTiled enc = get_encode();
   if (!enc) {
-    set_error("smot_conv2d(tcgen05): cuTensorMapEncodeTiled entry point not available");
+    set_error("smot_conv2d(wgmma): cuTensorMapEncodeTiled entry point not available");
     return false;
   }
   uint32_t estr[4] = {1, 1, 1, 1};
@@ -644,17 +646,16 @@ static bool encode_map(CUtensorMap* tm, const void* base, int rank, const uint64
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
-    set_error("smot_conv2d(tcgen05): cuTensorMapEncodeTiled failed with CUresult %d", (int)r);
+    set_error("smot_conv2d(wgmma): cuTensorMapEncodeTiled failed with CUresult %d", (int)r);
     return false;
   }
   return true;
 }
 
 // Widest split of the K loop of a few-tile layer (levels 4 / 5, FC layers), finished by splitk_reduce_kernel.
-// SMOT_TC_MAXSPLIT=1..8 (SMOT_TC_NOSPLIT=1 is MAXSPLIT=1).  Measured on B200 in the clip pipeline (profiles/bench_r02m_*.json):
-// splitting 8 ways makes the static stage ALONE faster (0.646 vs 0.658 ms) but the pipeline slower (1228 vs 1277 frames/s):
-// 8 CTAs per tile plus a 960-CTA reduce kernel per layer occupy SMs that the detection tail and the track stage of the
-// neighbouring frames would otherwise use.
+// SMOT_TC_MAXSPLIT=1..8 (SMOT_TC_NOSPLIT=1 is MAXSPLIT=1).  A wider split makes a layer alone faster, but 8 CTAs per
+// tile plus a reduce kernel per layer occupy SMs that the detection tail and the track stage of the neighbouring frames
+// would otherwise use.
 static int tc_max_split() {
   static const int v = [] {
     if (getenv("SMOT_TC_NOSPLIT")) return 1;
@@ -700,18 +701,18 @@ static cudaError_t launch_tc_ex(const CUtensorMap& tmA, const CUtensorMap& tmB, 
 template <int BN, int STAGES>
 static int launch_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, const TcArgs& a, dim3 grid, cudaStream_t st) {
   using S = TcSmem<BN, STAGES>;
-  SMOT_ENSURE_SMEM((conv_tc_kernel<BN, STAGES>), S::TOTAL, "smot_conv2d(tcgen05)");
+  SMOT_ENSURE_SMEM((conv_tc_kernel<BN, STAGES>), S::TOTAL, "smot_conv2d(wgmma)");
   cudaError_t e = launch_tc_ex<BN, STAGES>(tmA, tmB, a, grid, a.cluster_reduce ? a.splits : 1, st);
   if (e != cudaSuccess) {
-    set_error("smot_conv2d(tcgen05): launch failed: %s", cudaGetErrorString(e));
+    set_error("smot_conv2d(wgmma): launch failed: %s", cudaGetErrorString(e));
     return SMOT_ERR_CUDA;
   }
-  SMOT_CHECK_LAUNCH("smot_conv2d(tcgen05)");
+  SMOT_CHECK_LAUNCH("smot_conv2d(wgmma)");
   return SMOT_OK;
 }
 
 // How many (1,1,cz) clusters of this kernel variant the device can hold at once (a cluster lives inside one GPC, so this is
-// NOT 148 / cz: 8-CTA clusters fit twice into a 16..20-SM GPC).  Queried once per (variant, cz); 0 = query failed.
+// NOT sm_count() / cz: a GPC holds only a few clusters of 8).  Queried once per (variant, cz); 0 = query failed.
 template <int BN, int STAGES>
 static int tc_max_clusters(int cz) {
   static std::mutex mu;
@@ -751,9 +752,9 @@ static int tc_stages(int BN, bool solo, bool shallow, int my_chunks, int forced)
 template <int BN, int PW, int SB>
 static int launch_halo(const CUtensorMap& tmA, const CUtensorMap& tmB, const TcArgs& a, dim3 grid, int bo_mode, cudaStream_t st) {
   using S = HaloSmem<BN, PW, SB>;
-  SMOT_ENSURE_SMEM((conv3x3_halo_kernel<BN, PW, SB>), S::TOTAL, "smot_conv2d(tcgen05 halo)");
+  SMOT_ENSURE_SMEM((conv3x3_halo_kernel<BN, PW, SB>), S::TOTAL, "smot_conv2d(wgmma halo)");
   launch_pdl(conv3x3_halo_kernel<BN, PW, SB>, grid, dim3(TC_THREADS), S::TOTAL, st, tmA, tmB, a, bo_mode);
-  SMOT_CHECK_LAUNCH("smot_conv2d(tcgen05 halo)");
+  SMOT_CHECK_LAUNCH("smot_conv2d(wgmma halo)");
   return SMOT_OK;
 }
 
@@ -781,7 +782,7 @@ static int conv2d_tc_halo(const smot_conv_desc* d, int mode, cudaStream_t st) {
     const int bw = d->Cout % 256 == 0 ? 256 : (d->Cout % 128 == 0 ? 128 : 64);
     const long long cw = tiles * (d->Cout / bw);
     if (d->workspace && cw <= 40 && a.cin_chunks >= 2 && tc_max_split() > 1) {
-      int sp = (int)(148 / cw);
+      int sp = (int)(SMOT_TC_SPLIT_BASIS / cw);
       if (sp > tc_max_split()) sp = tc_max_split();
       if (sp > a.cin_chunks) sp = a.cin_chunks;
       const size_t need = (size_t)SMOT_CONV_WS_COUNTER_BYTES + (size_t)sp * tiles * TC_BM * d->Cout * sizeof(float);
@@ -806,11 +807,11 @@ static int conv2d_tc_halo(const smot_conv_desc* d, int mode, cudaStream_t st) {
   a.splits = (a.cin_chunks + a.chunks_per_split - 1) / a.chunks_per_split;
   a.num_tiles = (int)tiles;
   a.cluster_reduce = 0;
-  a.slices = 1, a.tmem_cols = 0;
+  a.slices = 1;
   a.dbg = nullptr;
   a.partial = d->workspace ? (float*)((char*)d->workspace + SMOT_CONV_WS_COUNTER_BYTES) : nullptr;
   dim3 grid((unsigned)tiles, (unsigned)(d->Cout / BN), (unsigned)a.splits);
-  const bool crowded = (long long)grid.x * grid.y * grid.z > 148;   // several CTAs per SM: shallow weight ring, 2 CTAs / SM
+  const bool crowded = (long long)grid.x * grid.y * grid.z > sm_count();   // several CTAs per SM: shallow weight ring, 2 CTAs / SM
   int rc;
 #define SMOT_HALO(BN_, SB_) (pw == 10 ? launch_halo<BN_, 10, SB_>(tmA, tmB, a, grid, bo_mode, st) : launch_halo<BN_, 16, SB_>(tmA, tmB, a, grid, bo_mode, st))
   if (BN == 256) rc = SMOT_HALO(256, 4);
@@ -838,10 +839,9 @@ int conv2d_tc(const smot_conv_desc* d, cudaStream_t st) {
   }
   a.tiles_w = ceil_div(d->OW, a.tile_w), a.tiles_h = ceil_div(d->OH, a.tile_h);
   const long long tiles = (long long)a.tiles_w * a.tiles_h * d->batch;
-  // Tile shape.  Measured (profiles/conv_probe_r01.txt): the k-steps issue at the tensor-pipe floor, but two thirds of a layer
-  // is per-kernel / per-CTA fixed cost (launch, TMEM allocation, epilogue).  Hence: (a) the widest N that still leaves ~100
-  // CTAs; (b) layers with only a handful of output tiles (levels 4-5, FC layers) take the widest BN AND split K over up
-  // to 8 CTAs, finished by splitk_reduce_kernel (not splitting, or splitting less, measured slower).
+  // Tile shape.  Most of these layers are short, so per-kernel / per-CTA fixed cost (launch, prologue, epilogue) is a large
+  // share of a layer.  Hence: (a) the widest N that still leaves ~100 CTAs; (b) layers with only a handful of output tiles
+  // (levels 4-5, FC layers) take the widest BN AND split K over up to 8 CTAs, finished by splitk_reduce_kernel.
   const int all_chunks = a.taps * a.cin_chunks;
   static const int min_ctas = getenv("SMOT_TC_MINCTAS") ? atoi(getenv("SMOT_TC_MINCTAS")) : 96;   // developer override
   int BN = 64;
@@ -850,9 +850,8 @@ int conv2d_tc(const smot_conv_desc* d, cudaStream_t st) {
   const char* force = getenv("SMOT_TC_STAGES");  // developer override: ring depth
   const int fs = force ? atoi(force) : 0;
   // developer switch SMOT_TC_CLUSTER=1: the split CTAs of a tile form a cluster and finish the tile themselves (tc_splitk_finish).
-  // Measured on B200 (profiles/bench_r02c_*): correct (bit-identical to the reduce kernel) but SLOWER -- 18.7-25.9 us per
-  // level-4 layer against 13.7 us + a 6 us reduce launch that overlaps the next layer's prologue through PDL; the serial
-  // store -> fence -> cluster barrier -> 128 KB read-back of one CTA cannot match a reduce grid that spreads over all SMs.
+  // Bit-identical to the reduce kernel, but the serial store -> fence -> cluster barrier -> 128 KB read-back of one CTA
+  // competes with a reduce grid that spreads over all SMs and overlaps the next layer's prologue through PDL.
   static const bool cluster_ok = getenv("SMOT_TC_CLUSTER") && atoi(getenv("SMOT_TC_CLUSTER")) == 1;
   int splits = 1, cluster_reduce = 0;
   {
@@ -863,7 +862,7 @@ int conv2d_tc(const smot_conv_desc* d, cudaStream_t st) {
     const long long tiles_img = tiles / (d->batch > 0 ? d->batch : 1);
     const long long cw = tiles_img * (d->Cout / bw);
     if (d->workspace && cw <= 40 && all_chunks >= 16 && tc_max_split() > 1) {
-      int sp = (int)(148 / cw);
+      int sp = (int)(SMOT_TC_SPLIT_BASIS / cw);
       if (sp > tc_max_split()) sp = tc_max_split();
       if (sp > all_chunks / 4) sp = all_chunks / 4;
       const size_t need = (size_t)SMOT_CONV_WS_COUNTER_BYTES + (size_t)sp * tiles * TC_BM * d->Cout * sizeof(float);
@@ -888,24 +887,19 @@ int conv2d_tc(const smot_conv_desc* d, cudaStream_t st) {
       }
     }
   }
-  // In-CTA K slices (developer switch SMOT_TC_SLICED=1 | 128 | 256 = N tile; default off): the SAME K ranges, summed in the SAME
-  // order -- bit-identical results (test_conv2d_tcgen05_k_slices_equal_split_k) -- but by one CTA with one TMEM accumulator per
-  // range (BN x slices <= 512 columns), no partial tiles, no reduce kernel.  Measured pairwise on the same boxes
-  // (profiles/bench_r02{r,s,t}_*.json; value / e2e frames/s, split -> sliced): 720p30 1243 / 1221 -> 1261 / 1262 (+1.5 / +3.4 %),
-  // but 1080p80 801 / 785 -> 785 / 770, R-50 570 / 608 -> 572 / 582, model(frame) 687 -> 663; slicing only the 8-wide splits
-  // (SMOT_TC_SLICED_MIN=8) lost on all three.  The split's extra CTAs fill the GPU where the neighbouring stages leave room and
-  // crowd it where they do not; with no rule that holds across the three workloads, the validated split path stays the default.
+  // In-CTA K slices (developer switch SMOT_TC_SLICED=1 | 128 = N tile; default off): the SAME K ranges, summed in the SAME
+  // order -- bit-identical results (test_conv2d_tcgen05_k_slices_equal_split_k) -- but by one CTA that adds each range's
+  // register accumulator to a running sum, no partial tiles, no reduce kernel.  The accumulator and the sum must both fit in
+  // registers, so N tiles stop at 128.  The split's extra CTAs fill the GPU where the neighbouring stages leave room and
+  // crowd it where they do not, so the split path stays the default.
   bool sliced = false;
   static const int slice_min = getenv("SMOT_TC_SLICED_MIN") ? atoi(getenv("SMOT_TC_SLICED_MIN")) : 2;
   if (splits >= slice_min && splits > 1 && !cluster_reduce) {
     const char* e = getenv("SMOT_TC_SLICED");
     if (e && e[0] != '0') {
-      int want = atoi(e);
-      if (want != 128 && want != 256) want = 64;
-      int bn = 512 / splits;                       // splits <= 8 -> >= 64
-      if (bn > BN) bn = BN;
-      if (bn > want) bn = want;
-      if (bn >= 64) sliced = true, BN = bn >= 256 ? 256 : (bn >= 128 ? 128 : 64);
+      const int want = atoi(e) == 128 ? 128 : 64;
+      const int bn = BN < want ? BN : want;
+      if (bn >= 64) sliced = true, BN = bn;
     }
   }
   CUtensorMap tmA, tmB;
@@ -928,12 +922,9 @@ int conv2d_tc(const smot_conv_desc* d, cudaStream_t st) {
   a.chunks_per_split = (all_chunks + splits - 1) / splits;
   a.splits = (all_chunks + a.chunks_per_split - 1) / a.chunks_per_split;  // no empty split
   a.cluster_reduce = (cluster_reduce && a.splits == splits) ? 1 : 0;
-  a.slices = 1, a.tmem_cols = 0;
+  a.slices = 1;
   if (sliced) {
     a.slices = a.splits, a.splits = 1;
-    int cols = 32;
-    while (cols < a.slices * BN) cols <<= 1;
-    a.tmem_cols = cols;
   }
   a.num_tiles = (int)tiles;
   {
@@ -942,12 +933,12 @@ int conv2d_tc(const smot_conv_desc* d, cudaStream_t st) {
   }
   a.partial = d->workspace ? (float*)((char*)d->workspace + SMOT_CONV_WS_COUNTER_BYTES) : nullptr;
   dim3 grid((unsigned)tiles, (unsigned)(d->Cout / BN), (unsigned)a.splits);
-  // many short tiles: 2-stage rings let 4 CTAs share an SM, so one CTA's prologue / epilogue overlaps the
-  // main loops of the others (same bytes in flight per SM as 2 CTAs x 4 stages)
+  // many short tiles: 2-stage rings let 2 CTAs share an SM, so one CTA's prologue / epilogue overlaps the
+  // main loops of the others (the same bytes in flight per SM as one CTA with 4 stages)
   const bool shallow = fs ? fs == 2 : (tiles * (d->Cout / BN) >= 296 && all_chunks <= 36);
-  // at most one CTA per SM: nothing else hides the ~1 us TMA round trip (the loop then advances `ring depth` chunks
+  // at most one CTA per SM: nothing else hides the TMA round trip (the loop then advances `ring depth` chunks
   // per round trip), so use the whole shared memory for the ring: 8 x 24 KB, 6 x 32 KB, 4 x 48 KB
-  const bool solo = (long long)grid.x * grid.y * grid.z <= 148;
+  const bool solo = (long long)grid.x * grid.y * grid.z <= sm_count();
   int stages = tc_stages(BN, solo, shallow, sliced ? all_chunks : a.chunks_per_split, fs);
   if (sliced && stages == 2) stages = BN == 128 ? 3 : 4;   // the 2-stage variants carry no slice code
 #define SMOT_TC_LAUNCH(BN_, ST_) launch_tc<BN_, ST_>(tmA, tmB, a, grid, st)

@@ -226,7 +226,7 @@ __device__ __forceinline__ void xm_mma_k8(float* c, uint32_t a0, uint32_t a1, ui
 // ---------------------------------------------------------------------------------------------
 // Planar-input form of the tensor-core correlation (developer switch SMOT_XCORR_PLANAR, see DESIGN.md section 5.2).
 //
-// ncu on xcorr_mma_kernel (profiles/ncu_xcorr_mma_r01_v12_raw.csv) puts the time in the window staging, not in the MMAs:
+// ncu on xcorr_mma_kernel puts the time in the window staging, not in the MMAs:
 // 21.6 k global load requests touching 25 sectors each (a warp gathers 30 x 16 B at a 256-byte stride; every sector is
 // requested twice), long-scoreboard + LSU-throttle stalls on 60 % of the issue slots, tensor pipe at 17 % of its rate.
 // Here the search windows arrive CHANNEL-PLANAR from smot_roi_align_planar -- per (track, channel) a plane of
@@ -319,7 +319,7 @@ __device__ __forceinline__ void xp_plane_mma(const __half* xw, const __half* kw,
   const int par = g & 1;
   const uint32_t a_s = (uint32_t)__cvta_generic_to_shared(xw + a_row * XM_PITCH + a_kh * 8);
   // the two copies of a template row sit 64 B apart: lanes with par = 0 / 1 read disjoint bank halves (conflict-free; a
-  // pair-interleaved image with 64-bit loads was measured SLOWER: both copies then alias the same banks, profiles/xcorr_lab_r02i_*)
+  // pair-interleaved image with 64-bit loads was measured SLOWER: both copies then alias the same banks)
   const uint32_t* kzw = reinterpret_cast<const uint32_t*>(kw + par * XM_KROW) + ((8 + 2 * t - g - par) >> 1);
 #pragma unroll
   for (int j = 0; j < 2; ++j)
@@ -499,10 +499,10 @@ __global__ void __launch_bounds__(XpGeom<CG>::THREADS) xcorr_planar_kernel(const
 }
 
 // ---------------------------------------------------------------------------------------------
-// Flat form of the planar kernel for launches that fit ONE wave (n * C <= 28 planes per SM; 30 tracks x 128 channels = 25.9).
+// Flat form of the planar kernel for launches that fit ONE wave (n * C <= 28 planes per SM).
 // (Developer variant, measured SLOWER than the 16-plane CTAs -- see xcorr_flat_enabled() -- and therefore not the default.)
-// With 16 planes per CTA, 3840 planes are 240 CTAs on 148 SMs: 92 SMs run 32 planes, 56 run 16, and the launch ends with the
-// loaded ones (trace: MMA phase 1.2 us on the light SMs, up to 3.3 us on the others).  Here the plane list is cut into 4-plane
+// With 16 planes per CTA, 3840 planes are 240 CTAs on 132 SMs: 108 SMs run 32 planes, 24 run 16, and the launch ends with the
+// loaded ones.  Here the plane list is cut into 4-plane
 // units (a unit never straddles a track or an 8-byte channel vector) and CTA b of gridDim.x takes units
 // [b * U / grid, (b + 1) * U / grid): 24 or 28 planes on EVERY SM, one CTA per SM, one MMA warp per plane (up to 28 + the copy
 // warp).  Templates and results move as 8-byte vectors (a unit's four channels).  Per-plane arithmetic is xp_plane_mma's, so the
@@ -872,10 +872,8 @@ static bool xcorr_planar_trimmed() {
   return on;
 }
 
-// planes per CTA.  Measured ladder (B200, CUDA-graph replay, us per launch; profiles/xcorr_lab_r02h.json):
-//   30 tracks x 128 ch (3840 planes):  16: 6.15   8: 7.55   4: 7.93   2: 9.71
-//   80 tracks x 128 ch (10240 planes): 16: 14.31  8: 13.33  4: 15.91  2: 22.18       30 x 256 ch: 16: 11.60  8: 10.65
-// i.e. 16 while all CTAs are resident at once (two per SM), 8 beyond that.  Developer switch SMOT_XCORR_CG (read once).
+// planes per CTA: 16 while all CTAs are resident at once (two per SM), 8 beyond that (the fastest of 2 / 4 / 8 / 16 at
+// 30 and 80 tracks when it was chosen; not re-measured on the H100).  Developer switch SMOT_XCORR_CG (read once).
 static int xcorr_planar_cg(int planes) {
   static const int forced = [] {
     const char* e = getenv("SMOT_XCORR_CG");
@@ -891,7 +889,7 @@ extern "C" int smot_xcorr_planar(const void* x_planar, const void* k, void* out,
 }
 
 // developer switch SMOT_XCORR_FLAT=1 (read once): the flat form whenever the planes fit one wave of 28 per SM.  OFF by default:
-// measured 7.34 us against 5.80 us for 16-plane CTAs at 30 x 128 (profiles/bench_r02l_*.json) -- the balance it buys (28 instead
+// measured slower than 16-plane CTAs at 30 x 128 when it was written -- the balance it buys (28 instead
 // of 32 planes on the busiest SM) is worth less than what one 29-warp CTA per SM loses: its phases (template staging, wait for
 // the windows, MMA, result path) cannot overlap with those of a second CTA, its block barriers span 928 threads, and templates /
 // results move as 8-byte instead of 16-byte vectors.

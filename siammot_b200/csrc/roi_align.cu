@@ -189,7 +189,7 @@ __global__ void __launch_bounds__(256) roi_align_planar_kernel(const RoiArgs a, 
 // ---------------------------------------------------------------------------------------------
 // Row-wise ROIAlign with separable sample tables (round 2).
 //
-// ncu on the kernels above (profiles/ncu_roi_align_planar_r02.txt): 27 M warp instructions for 27 000 bins, issue slots 75 %
+// ncu on the kernels above: 27 M warp instructions for 27 000 bins, issue slots 75 %
 // busy, L1 hit rate 80 %, DRAM 2 % -- they are INSTRUCTION bound: every warp re-derives the level (log2 / sqrt / IEEE
 // division), the bin geometry (4 divisions) and, per sample, two IEEE divisions plus ~40 instructions of clamping and
 // bounds logic, ~1000 instructions per bin of which ~150 are loads and multiply-adds.

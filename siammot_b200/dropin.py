@@ -2,7 +2,7 @@
 
 The reference's drivers obtain the model through one name -- ``from siammot.modelling.rcnn import build_siammot``
 (demos/demo_inference.py:13, tools/test_net.py:13, used at demo_inference.py:85 / test_net.py:39).  ``install()`` registers a
-module under that name whose ``build_siammot`` is the B200 engine's, BEFORE the reference's own module is imported, so the
+module under that name whose ``build_siammot`` is the engine's, BEFORE the reference's own module is imported, so the
 reference's ``DemoInference`` / ``DatasetInference`` / ``do_inference`` run on the engine without a single edited line:
 
     SIAMMOT_ENGINE=b200 python -c "import siammot_b200.dropin" demos/demo.py ...        # or: import siammot_b200.dropin at start-up

@@ -1,6 +1,6 @@
 """Per-frame execution engine: weight preparation, static launch plan, dynamic tracker stage.
 
-This is the B200-native replacement for everything beneath ``SiamMOT.forward``
+This is the H100 (sm_90a) replacement for everything beneath ``SiamMOT.forward``
 (/root/reference/siammot/modelling/rcnn.py:41-68).  Design:
 
 * activations live in NHWC device buffers allocated once per input resolution; DLA roots read their
@@ -16,7 +16,7 @@ This is the B200-native replacement for everything beneath ``SiamMOT.forward``
 * exactly one device->host copy per frame (the solver needs ids on the host, track_solver.py:62-106),
   against >= 10 hidden syncs in the reference (SURVEY.md section 3.3).
 
-All compute is libsmot.so (hand-written sm_100a CUDA); torch is used for memory, streams, graphs and
+All compute is libsmot.so (hand-written sm_90a CUDA for the H100); torch is used for memory, streams, graphs and
 a few single-element glue ops on tiny tensors.  No CPU fallback exists.
 """
 import ctypes as C
@@ -514,11 +514,11 @@ class Engine(object):
         try:
             return torch.cuda.get_device_properties(self.device).multi_processor_count
         except Exception:      # no CUDA runtime (the host-side emulation tests)
-            return 148
+            return 132
 
     def __init__(self, cfg, device="cuda", dtype=None, use_graph=True):
         if not torch.cuda.is_available():
-            raise RuntimeError("siammot_b200 needs a CUDA device (sm_100a); there is no CPU path")
+            raise RuntimeError("siammot_b200 needs an sm_90a CUDA device (H100); there is no CPU path")
         lib()  # fail loudly if the CUDA library is missing
         self.cfg = cfg
         self.device = torch.device(device)
@@ -581,10 +581,10 @@ class Engine(object):
         # on a third stream under the backbone of frame t+1; SMOT_CLIP_SLOTS = number of static-plan copies (2 or 3)
         self.body_branches = os.environ.get("SMOT_BODY_BRANCHES", "0") == "1"
         # SiamMOT.forward: detection tail of the frame on a second stream under the EMM half of its track stage
-        # (default since round 2: measured 639 vs 580 FPS per-frame on the driver's B200, identical tracks; =0 restores the serial order)
+        # (default; identical tracks; =0 restores the serial order)
         self.frame_overlap = os.environ.get("SMOT_FRAME_OVERLAP", "1") == "1"
         # forward_clip: three-stage pipeline over 3 static-plan copies by default (round 2: measured 989 / 1071 FPS value / e2e
-        # against 900 / 946 for the two-stream pipeline on the driver's B200, identical tracks); SMOT_CLIP_SPLIT=0 = two-stream
+        # faster than the two-stream pipeline on earlier hardware, identical tracks); SMOT_CLIP_SPLIT=0 = two-stream
         self.clip_split = os.environ.get("SMOT_CLIP_SPLIT", "1") == "1"
         self.clip_slots = max(2, min(4, int(os.environ.get("SMOT_CLIP_SLOTS", "3"))))
         self._pre = None
@@ -595,7 +595,6 @@ class Engine(object):
         # SMOT_CLIP_SLOTS >= streams + 1 plan copies to matter)
         self.clip_backbone_streams = max(1, min(3, int(os.environ.get("SMOT_CLIP_BACKBONE_STREAMS", "1"))))
         # forward_clip (three-stage): backbone half over frame pairs (Engine.pair_plan); SMOT_CLIP_PAIRS=0 = one frame per pass
-        # (measured on B200, profiles/bench_r02f_*: 1204 vs 1168 FPS device-resident, 1171 vs 1126 from host frames)
         self.clip_pairs = os.environ.get("SMOT_CLIP_PAIRS", "1") == "1"
         # forward_clip: the host work nothing waits for (result BoxList, per-id cache update) runs under the NEXT frame's track
         # stage instead of in front of it (SMOT_CLIP_DEFER=0: in line, as model(frame) does)
@@ -603,7 +602,7 @@ class Engine(object):
         # forward_clip (three-stage): the backbone / detection-tail enqueues (graph launches, input copies) and the deferred
         # host work run on a helper thread, so the caller's thread only carries the sequential chain of a video
         # (track stage launch -> wait -> solver -> next memory).  SMOT_CLIP_THREAD=0: everything on the caller's thread.
-        # Measured on B200 (profiles/bench_r02f_*): SLOWER and noisier (1082 +- 70 vs 1168 FPS) -- the clip is bound by the GPU
+        # Measured slower and noisier on earlier hardware -- the clip is bound by the GPU
         # (backbone + detection tail + track stage co-scheduled: 0.86 ms per frame), the time the caller's thread saves only
         # moves into its wait for the track stage, and two Python threads contend for the GIL.  Off by default.
         self.clip_thread = os.environ.get("SMOT_CLIP_THREAD", "0") == "1"
@@ -616,7 +615,7 @@ class Engine(object):
         # smot_xcorr_planar).  Off by default until it has been through the GPU tests.
         self.nvtx = os.environ.get("SMOT_NVTX", "0") == "1"
         # channel-planar search-window exchange (default since round 2: bit-equal windows, 1.5-2x faster correlation on the
-        # driver's B200); 0 = NHWC windows + xcorr_mma_kernel, 1 = planar with the untrimmed MMA phase, 2 = trimmed (libsmot reads it)
+        # earlier hardware); 0 = NHWC windows + xcorr_mma_kernel, 1 = planar with the untrimmed MMA phase, 2 = trimmed (libsmot reads it)
         self.xcorr_planar = os.environ.get("SMOT_XCORR_PLANAR", "2") in ("1", "2")
         self.xcorr_planar_mode = 0 if os.environ.get("SMOT_XCORR_PLANAR", "2") == "1" else 1   # the engine passes it per call
         self.timers = None  # optional dict name -> list of (start_event, end_event), see timed()
@@ -925,8 +924,8 @@ class Engine(object):
     def pair_plan(self, H, W, pslot=0):
         """Backbone plan over a PAIR of clip frames (batch 2) + the two per-frame plans that read its halves.
 
-        Below level 2 every DLA / FPN / RPN layer has at most 110..120 CTAs for 148 SMs and costs ~10 us whatever its size
-        (launch, barrier + TMEM setup, TMA round trips, epilogue -- profiles/): run over two frames at once those layers cost
+        Below level 2 every DLA / FPN / RPN layer has at most 110..120 CTAs for the 132 SMs of an H100 and costs ~10 us whatever its size
+        (launch, barrier setup, TMA round trips, epilogue): run over two frames at once those layers cost
         the same and do twice the work, only the layers that already fill the GPU (stem, level 0-2, P2) double.
         forward_clip's three-stage mode therefore runs the backbone half of frames (2k, 2k+1) as ONE batch-2 pass; the
         detection tail and the track stage stay per frame and read image i of the batched buffers through the frame plans

@@ -875,7 +875,7 @@ def _join(events, enq):
 
 def _forward_clip_pairs(self, eng, frames, before_frame=None, given_detections=None):
     """The three-stage clip pipeline with the backbone half run over frame PAIRS (Engine.pair_plan: one batch-2 pass for
-    frames 2k, 2k+1 -- the layers below level 2 do not fill 148 SMs with one frame and cost the same for two).
+    frames 2k, 2k+1 -- the layers below level 2 do not fill the GPU's SMs with one frame and cost the same for two).
 
       stream A   B(2k, 2k+1): input copies / test transform of both frames, ONE batch-2 backbone + FPN + RPN-head pass
       stream D   D(t): proposal selection, box head, per-class NMS of frame t (its image of the batched buffers)

@@ -1,7 +1,7 @@
 """Tensor-level wrappers over the C ABI (include/smot.h).
 
 PyTorch is used for what it is here for: device memory, streams.  Every function launches
-hand-written sm_100a kernels from libsmot.so on the current CUDA stream and raises RuntimeError on
+hand-written sm_90a kernels from libsmot.so on the current CUDA stream and raises RuntimeError on
 failure; none has a CPU or torch-op fallback.
 
 Activations are NHWC tensors (B, H, W, C); a channel slice ``buf[..., a:b]`` of a wider buffer is a

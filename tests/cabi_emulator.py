@@ -6,7 +6,7 @@ per-frame path calls is emulated here with the oracle's primitives on the very p
 the CUDA runtime objects the engine uses for ordering (streams, events) become no-ops.  An end-to-end run through this
 emulation reproduces the reference goldens iff the host logic wires the calls correctly (tests/test_engine_emulated_cpu.py).
 What it does NOT test is the CUDA kernels: those are compared with the same oracle primitives, per op and end to end, by the
-`-m gpu` tests on a B200.
+`-m gpu` tests on an H100.
 """
 import contextlib
 import ctypes as C

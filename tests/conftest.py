@@ -10,7 +10,7 @@ for p in (REPO, os.path.join(REPO, "tests")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box: pytest -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100: pytest -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):

@@ -261,7 +261,7 @@ OUT_HIRES = os.path.join(HERE, "_hires_cpu.so")
 
 
 def generate_hires():
-    """csrc/conv_hires.cu: the per-tile kernels of the stem / level0 (validated on the B200 against the oracle) and their
+    """csrc/conv_hires.cu: the per-tile kernels of the stem / level0 (validated on the GPU against the oracle) and their
     persistent forms, over shim_tc.h (cp.async = immediate copy or zero fill, ldmatrix / mma.sync emulated).  The persistent
     kernels must reproduce the per-tile ones bit for bit."""
     src = open(os.path.join(CSRC, "conv_hires.cu")).read()

@@ -7,7 +7,7 @@
 //                                                 b0 (k = 2t.., n = g) b1 (k = 2t+8.., n = g); c0 c1 (g, 2t 2t+1) c2 c3 (g+8, ..)
 //   mbarrier.init / arrive.expect_tx / try_wait.parity, cp.async.bulk.shared.global with complete_tx (one phase)
 // Shared-memory "addresses" are byte offsets into the shim's dynamic shared-memory buffer, as on the GPU.
-// xcorr_mma_kernel -- validated on the B200 -- runs through the same emulation, which is what validates the emulation.
+// xcorr_mma_kernel -- validated on the GPU -- runs through the same emulation, which is what validates the emulation.
 #pragma once
 #define SHIM_WITH_CUDA_FP16
 #include "shim.h"

@@ -1,3 +1,4 @@
+import gzip
 import os
 
 import torch
@@ -10,6 +11,36 @@ from siammot_b200.synth_clip import make_clip
 CONFIG_DIR = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "siammot_b200", "configs")
 YAML_MAP = {"DLA_34_FPN_EMM.yaml": "dla34_emm.yaml", "DLA_34_FPN_EMM_MOT17.yaml": "dla34_emm_mot17.yaml",
             "DLA_34_FPN_EMM_AOT.yaml": "dla34_emm_aot.yaml"}
+
+
+REFERENCE_VECTORS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_vectors.pt.gz")
+
+
+def ref_vectors():
+    """What the reference's own modules produced for the seeded inputs of the tests (tests/golden/make_reference_vectors.py)."""
+    with gzip.open(REFERENCE_VECTORS, "rb") as f:
+        return torch.load(f)
+
+
+def sample_index(numel, n=256):
+    """The fixed sample of element positions stored for a tensor of `numel` elements (seeded by its size)."""
+    g = torch.Generator().manual_seed(numel)
+    return torch.randint(0, numel, (min(n, numel),), generator=g)
+
+
+def assert_matches_sample(t, ref, rel=None):
+    """`t` against a stored sample of the reference's tensor: shape, the sampled elements and the float64 sums; bit-exact unless
+    `rel` (a bound relative to the reference's largest magnitude) is given."""
+    assert tuple(t.shape) == tuple(ref["shape"]), (tuple(t.shape), ref["shape"])
+    flat = t.detach().reshape(-1).float()
+    got = flat[sample_index(flat.numel())]
+    if rel is None:
+        assert torch.equal(got, ref["val"])
+        assert float(flat.double().sum()) == ref["sum"] and float(flat.double().abs().sum()) == ref["abs_sum"]
+    else:
+        bound = rel * ref["abs_max"]
+        assert float((got - ref["val"]).abs().max()) <= bound
+        assert abs(float(flat.double().sum()) - ref["sum"]) <= bound * flat.numel()
 
 
 def _spec(name):

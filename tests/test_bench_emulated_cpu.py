@@ -84,3 +84,48 @@ def test_demo_clip_tool_end_to_end(monkeypatch, tmp_path):
     recs = json.loads(out.read_text())
     assert len(recs) == len(kept) and all(set(r) == {"frame_num", "id", "label", "confidence", "bbox"} for r in recs)
     assert all(r["id"] >= 0 and len(r["bbox"]) == 4 for r in recs)
+
+
+def test_bench_dump_outputs_are_typed_and_repeatable(monkeypatch, tmp_path):
+    """`--dump-outputs DIR`: the last timed step's result arrays as float32 / float64 .npy files, equal from run to run."""
+    import numpy as np
+    cabi_emulator.install_for_bench(monkeypatch)
+    import bench
+    dumps = []
+    for run in range(2):
+        d = tmp_path / ("run%d" % run)
+        monkeypatch.setattr(sys, "argv", ["bench.py", "--steps", "2", "--regions", "2", "--warmup", "3", "--dtype", "float32",
+                                          "--no-cpu-baseline", "--experimental", "off", "--workload", "selftest",
+                                          "--dump-outputs", str(d)])
+        buf = io.StringIO()
+        try:
+            with contextlib.redirect_stdout(buf):
+                bench.main()
+        finally:
+            bench.select_workload("720p30")
+        line = json.loads(buf.getvalue().strip().splitlines()[-1])
+        assert line["steps"] == 2 and len(line["spread"]["value_fps"]) == 2
+        dumps.append({p.name: np.load(p) for p in sorted(d.glob("*.npy"))})
+    assert {"boxes.npy", "scores.npy", "labels.npy", "ids.npy"} <= set(dumps[0]) and dumps[0].keys() == dumps[1].keys()
+    for name, a in dumps[0].items():
+        assert a.dtype in (np.float32, np.float64), (name, a.dtype)
+        assert np.array_equal(a, dumps[1][name]), name
+    assert dumps[0]["boxes.npy"].shape[1:] == (4,) and dumps[0]["boxes.npy"].shape[0] > 0
+
+
+def test_bench_reference_arm_dumps_its_last_step(monkeypatch, tmp_path):
+    """`--impl reference --dump-outputs DIR`: the oracle's last timed step under the same names, so two arms compare array by array."""
+    import numpy as np
+    import bench
+    monkeypatch.setattr(sys, "argv", ["bench.py", "--impl", "reference", "--steps", "1", "--warmup", "1", "--workload", "selftest",
+                                      "--dump-outputs", str(tmp_path)])
+    buf = io.StringIO()
+    try:
+        with contextlib.redirect_stdout(buf):
+            bench.main()
+    finally:
+        bench.select_workload("720p30")
+    assert json.loads(buf.getvalue().strip().splitlines()[-1])["steps"] == 1
+    arrays = {p.name: np.load(p) for p in tmp_path.glob("*.npy")}
+    assert {"boxes.npy", "ids.npy"} <= set(arrays), sorted(arrays)
+    assert all(a.dtype in (np.float32, np.float64) for a in arrays.values())

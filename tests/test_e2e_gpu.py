@@ -1,4 +1,4 @@
-"""End-to-end parity of the B200 engine with the reference, through the drop-in API
+"""End-to-end parity of the engine with the reference, through the drop-in API
 (build_siammot(cfg) -> model(frame) -> [BoxList]), on the seeded scenarios whose expected outputs were
 produced by the reference's own code (tests/golden/*.pt).
 

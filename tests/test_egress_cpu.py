@@ -1,6 +1,7 @@
 """Clip-level result egress (siammot_b200/egress.py) against the reference's own code: ``boxlists_to_entities`` is imported
 verbatim (over stand-ins for gluoncv's two container classes), ``DatasetInference._postprocess_tracks`` is executed from its
-source text (its module needs motmetrics & co. to import).  Needs the reference tree (authoring container)."""
+source text (its module needs motmetrics & co. to import).  What they return for the seeded results below is stored by
+tests/golden/make_reference_vectors.py."""
 import ast
 import os
 import sys
@@ -10,9 +11,20 @@ import numpy as np
 import pytest
 import torch
 
-from oracle import reference_loader
+VIDEOS = [(1280, 720), (1920, 1080), (2560, 1408)]
 
-pytestmark = pytest.mark.skipif(not reference_loader.available(), reason="reference tree not present")
+
+def entity_tuple(e):
+    return (tuple(e.bbox), e.confidence, e.labels, e.id, e.frame_num, e.time)
+
+
+def entity_key(e):
+    return (e.id, e.frame_num, tuple(e.bbox))
+
+
+class PostprocessSelf(object):
+    """The two attributes DatasetInference._postprocess_tracks reads from its instance."""
+    _track_len, _track_conf = 5, 0.7
 
 
 def _random_results(seed, n_frames=12, net=(1280, 704)):
@@ -31,31 +43,23 @@ def _random_results(seed, n_frames=12, net=(1280, 704)):
     return out
 
 
-@pytest.mark.parametrize("video", [(1280, 720), (1920, 1080), (2560, 1408)])
+@pytest.mark.parametrize("video", VIDEOS)
 def test_clip_to_tracks_and_entities_equal_the_reference_path(video):
-    reference_loader.load()
-    from maskrcnn_benchmark.structures.bounding_box import BoxList as RefBoxList
-    from siammot.utils.boxlists_to_entities import boxlists_to_entities
+    from helpers import ref_vectors
     from siammot_b200 import egress
     results = _random_results(video[0])
-    # the reference path, per frame (inferencer.py:64-70)
-    ref_entities = []
-    for t, r in enumerate(results):
-        rb = RefBoxList(r.bbox.clone(), r.size, "xyxy")
-        for f in r.fields():
-            rb.add_field(f, r.get_field(f))
-        o = rb.resize([video[0], video[1]]).convert("xywh").to(torch.device("cpu"))
-        ref_entities += boxlists_to_entities([o], 100 + t, [0.04 * (100 + t)], class_table=["person", "vehicle"])
+    # the reference path, per frame (inferencer.py:64-70): BoxList.resize -> convert("xywh") -> boxlists_to_entities
+    ref_entities = ref_vectors()["egress"][video]
     tracks = egress.clip_to_tracks(results, video[0], video[1], first_frame_idx=100, timestamps=[0.04 * (100 + t) for t in range(len(results))])
     got = egress.to_entities(tracks, class_table=["person", "vehicle"])
     assert len(got) == len(ref_entities) == len(tracks)
-    for a, b in zip(got, ref_entities):
-        assert a.bbox == b.bbox and a.confidence == b.confidence and a.labels == b.labels
-        assert a.id == b.id and a.frame_num == b.frame_num and a.time == b.time
+    assert [entity_tuple(e) for e in got] == ref_entities
 
 
 def _reference_postprocess():
     """DatasetInference._postprocess_tracks, literally, from the reference file."""
+    from oracle import reference_loader
+    reference_loader.load()
     path = os.path.join(reference_loader.REFERENCE_ROOT, "siammot", "engine", "inferencer.py")
     src = open(path).read()
     tree = ast.parse(src)
@@ -72,19 +76,14 @@ def _reference_postprocess():
 
 
 def test_postprocess_tracks_equals_the_reference_filter():
-    reference_loader.load()
+    from helpers import ref_vectors
     from siammot_b200 import egress
-    fn, DataSample = _reference_postprocess()
-
-    class Self(object):
-        _track_len, _track_conf = 5, 0.7
     results = _random_results(7, n_frames=40)
     tracks = egress.clip_to_tracks(results, 1280, 720)
-    sample = DataSample("v", entities=egress.to_entities(tracks, ["person", "vehicle"]))
-    ref = fn(Self(), sample).entities
-    got = egress.to_entities(egress.postprocess_tracks(tracks, 5, 0.7), ["person", "vehicle"])
-    key = lambda e: (e.id, e.frame_num, tuple(e.bbox))
-    assert len(ref) > 0 and sorted(map(key, ref)) == sorted(map(key, got))
+    ref = ref_vectors()["egress"]["postprocess"]      # _postprocess_tracks(PostprocessSelf(), <these tracks>), sorted keys
+    got = egress.to_entities(egress.postprocess_tracks(tracks, PostprocessSelf._track_len, PostprocessSelf._track_conf),
+                             ["person", "vehicle"])
+    assert len(ref) > 0 and ref == sorted(map(entity_key, got))
     assert all(e.id >= 0 for e in got)
     # grouped by id, frames ascending
     assert [(e.id, e.frame_num) for e in got] == sorted((e.id, e.frame_num) for e in got)

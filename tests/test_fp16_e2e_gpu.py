@@ -1,4 +1,4 @@
-"""End-to-end parity of the BENCHMARKED arithmetic (DTYPE float16: tcgen05 / mma.sync convolutions, planar tensor-core
+"""End-to-end parity of the BENCHMARKED arithmetic (DTYPE float16: wgmma / mma.sync convolutions, planar tensor-core
 correlation) at the benchmarked geometry: 3x704x1280 network input, 30 tracks injected into the memory, 8 consecutive frames
 (and the 1080p / 80-track and R-50 variants of BASELINE.json configs[2] / [4]).
 
@@ -7,13 +7,12 @@ which also checks that the CPU oracle reproduces them and stores the oracle's de
 
 What can be demanded of fp16 storage through ~45 layers, and what this file asserts:
   * the scene is DECISIVE: every id-deciding comparison of the clip (detection threshold 0.05, both NMS 0.5 tests and score
-    orders, the solver's 0.4 / 0.6 thresholds -- tests/decisive.py) keeps a margin far above the fp16 deviation measured on a
-    B200.  The margins come from the fixture and are asserted first, so a scene that stops being decisive fails as such;
+    orders, the solver's 0.4 / 0.6 thresholds -- tests/decisive.py) keeps a margin far above the measured fp16 deviation.  The margins come from the fixture and are asserted first, so a scene that stops being decisive fails as such;
   * ids: on EVERY frame the engine returns exactly the reference's id set with the reference's labels, and the same number
     of untracked detections.  Rows are paired by id, not by position: the reference orders rows by score, and 30 tracks whose
     scores differ by less than the fp16 deviation have no reproducible order;
-  * boxes of paired rows within BOX_BOUND px, scores within SCORE_BOUND (measured on a B200 in round 2: 1.37 px / 0.021 on
-    full_720p30; the EMM arg-max sits on a smooth maximum of a 256x256 map, so an fp16 perturbation moves it by a grid step
+  * boxes of paired rows within BOX_BOUND px, scores within SCORE_BOUND (measured on an H100 80GB HBM3, 700 W: 0.665 px / 0.0212 on
+    full_720p30, DESIGN.md 2.1; the EMM arg-max sits on a smooth maximum of a 256x256 map, so an fp16 perturbation moves it by a grid step
     or two = 0.4-1.4 px of the search region, and the confidence read at the new position moves with it);
   * the float32 engine on the same clip stays at the north-star tolerance (ids in the reference's ORDER, boxes <= 1e-3 px).
 """
@@ -73,14 +72,17 @@ def _pair_and_check(gold_frames, got, box_bound, score_bound, ordered):
             kb = torch.tensor([oa[i] for i in sorted(ga)], dtype=torch.int64)
             assert torch.equal(g["labels"][ka], o["labels"][kb]), "frame %d: labels of paired tracks differ" % t
             gb, ob, gs, os_ = g["boxes"][ka], o["boxes"][kb], g["scores"][ka], o["scores"][kb]
-            # untracked detections (id -1): pair each reference row with the nearest engine row
+            # untracked detections (id -1): pair each reference row with the nearest engine row of the same label (one object
+            # yields a detection per class with nearly the same box, so the box alone does not identify the counterpart)
             gu, ou = (gi < 0).nonzero().squeeze(1), (oi < 0).nonzero().squeeze(1)
             assert gu.numel() == ou.numel(), "frame %d: %d untracked detections vs %d" % (t, ou.numel(), gu.numel())
             for r in gu.tolist():
-                d = (o["boxes"][ou] - g["boxes"][r]).abs().max(dim=1)[0]
+                cand = ou[o["labels"][ou] == g["labels"][r]]
+                assert cand.numel() > 0, "frame %d: no untracked detection of label %d" % (t, int(g["labels"][r]))
+                d = (o["boxes"][cand] - g["boxes"][r]).abs().max(dim=1)[0]
                 j = int(torch.argmin(d))
                 assert float(d[j]) <= box_bound, "frame %d: untracked detection without a counterpart (%.2f px)" % (t, float(d[j]))
-                assert abs(float(o["scores"][ou[j]] - g["scores"][r])) <= score_bound
+                assert abs(float(o["scores"][cand[j]] - g["scores"][r])) <= score_bound
         if gb.numel():
             worst_box = max(worst_box, float((gb - ob).abs().max()))
             worst_score = max(worst_score, float((gs - os_).abs().max()))

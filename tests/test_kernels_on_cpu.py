@@ -133,7 +133,7 @@ def cpu_xcorr():
 @pytest.mark.parametrize("n,Cc", [(2, 32), (1, 16), (3, 48)])
 def test_xcorr_kernels_source_under_ptx_emulation(cpu_xcorr, n, Cc):
     """csrc/emm.cu's tensor-core correlation kernels, source text, with ldmatrix / mma.sync / mbarrier / cp.async.bulk emulated
-    on the host (tests/cpu_cuda/shim_tc.h).  xcorr_mma_kernel is validated on the B200: its agreement with the oracle here
+    on the host (tests/cpu_cuda/shim_tc.h).  xcorr_mma_kernel is validated on the GPU: its agreement with the oracle here
     validates the emulation.  xcorr_planar_kernel (written without GPU access: bulk-copy staging from channel-planar windows,
     17th warp, mbarrier) must then reproduce xcorr_mma_kernel's output bit for bit."""
     from oracle import siammot_oracle as orc
@@ -259,7 +259,7 @@ def cpu_hires():
 
 @pytest.mark.parametrize("H,W,batch,ctas", [(100, 130, 1, 6), (40, 70, 2, 3)])
 def test_persistent_hires_kernels_reproduce_the_per_tile_kernels(cpu_hires, H, W, batch, ctas):
-    """csrc/conv_hires.cu: stem 7x7 3->16 and level0 3x3 16->16.  The per-tile kernels are validated on the B200 (oracle bar);
+    """csrc/conv_hires.cu: stem 7x7 3->16 and level0 3x3 16->16.  The per-tile kernels are validated on the GPU (oracle bar);
     here they also meet torch's convolution, which validates the emulation, and the persistent forms (weights as register-resident
     B fragments, a warp owns four output rows, double-buffered halo, several tiles per CTA, ragged right / bottom tiles, two
     images) must equal them bit for bit -- garbage in the output pitch's unused channels stays untouched."""

@@ -1,5 +1,5 @@
-"""Further GPU parity cases: more configuration switches, bodies and pipeline modes (all passed on the driver's B200 at the end
-of round 1 while still marked pending; promoted to plain tests in round 2, so a regression fails the suite).  Expected outputs
+"""Further GPU parity cases: more configuration switches, bodies and pipeline modes (plain tests, so a regression
+fails the suite).  Expected outputs
 come from the reference itself (tests/golden/make_golden.py, ORACLE_SCENARIOS); the CPU oracle is pinned to the same fixtures
 in tests/test_oracle_golden.py."""
 import pytest

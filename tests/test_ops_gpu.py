@@ -347,7 +347,7 @@ TC_CASES = [
 
 @pytest.mark.parametrize("case", TC_CASES)
 def test_conv2d_tcgen05_matches_oracle_and_simt(case):
-    """The tcgen05/TMA member of the conv family against torch fp32 on the fp16-rounded operands and
+    """The wgmma/TMA member of the conv family against torch fp32 on the fp16-rounded operands and
     against the SIMT member (same operands, fp32 accumulation in both)."""
     from siammot_b200 import _lib
     B, Cin, H, W, Cout, k, use_res, relu, use_scale = case
@@ -539,8 +539,8 @@ def test_conv2d_hires_persistent_kernels(case, monkeypatch):
 
 @pytest.mark.parametrize("mode", ["16", "10"])
 def test_conv2d_tcgen05_halo_variant(mode, monkeypatch):
-    """Developer variant of the 3x3 tcgen05 kernel (SMOT_TC_HALO): the input halo of an 8x16 tile stays in shared
-    memory and the nine taps are shifted UMMA descriptors over it (patch rows of 16 or 10 pixels).  Same results."""
+    """Developer variant of the 3x3 wgmma kernel (SMOT_TC_HALO): the input halo of an 8x16 tile stays in shared
+    memory and the nine taps are shifted wgmma descriptors over it (patch rows of 16 or 10 pixels).  Same results."""
     from siammot_b200 import _lib
     monkeypatch.setenv("SMOT_TC_HALO", mode)
     g = torch.Generator().manual_seed(int(mode))
@@ -594,7 +594,7 @@ def test_conv2d_tcgen05_split_k():
 @pytest.mark.parametrize("case", [(1, 512, 22, 40, 512, 3), (1, 256, 44, 80, 256, 3), (2, 256, 44, 80, 256, 3), (1, 1280, 22, 40, 512, 1),
                                   (1, 6272, 1, 300, 1024, 1), (1, 256, 22, 40, 512, 3), (1, 128, 16, 16, 256, 3)])
 def test_conv2d_tcgen05_k_slices_equal_split_k(case, monkeypatch):
-    """Few-tile layers: one CTA with one TMEM accumulator per K range (SMOT_TC_SLICED=1) against the split CTAs + reduce kernel
+    """Few-tile layers: one CTA that adds each K range's register accumulator to a running sum (SMOT_TC_SLICED=1) against the split CTAs + reduce kernel
     (the default): the same K ranges summed in the same order -- the same bits -- for levels 4 / 5, a root 1x1, fc6 and a batch
     of two (frame-pair plans)."""
     from siammot_b200 import _lib

@@ -1,4 +1,4 @@
-"""demos/demo.py for the B200 engine, minus video decoding and visualisation (both out of scope, DESIGN.md section 8):
+"""demos/demo.py for the engine, minus video decoding and visualisation (both out of scope, DESIGN.md section 8):
 decoded RGB uint8 frames in -> tracks out, through the calls a siam-mot user switches to.
 
     python tools/demo_clip.py --frames clip.npy --weights model.pth --out tracks.json        # (T, H, W, 3) uint8 frames

@@ -1,4 +1,4 @@
-"""Developer tool: phase timestamps (ns, %globaltimer) of CTA 0 of one tcgen05 conv launch."""
+"""Developer tool: phase timestamps (ns, %globaltimer) of CTA 0 of one wgmma conv launch."""
 import math, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -1,6 +1,6 @@
 """Developer tool: per-kernel SASS opcode histogram of libsmot.so (cuobjdump -sass), the mnemonics that prove which hardware paths
-a kernel uses (tcgen05: UTCHMMA / UTCBAR / UTCATOMSWS, TMEM loads: LDTM, TMA: UTMALDG / UBLKCP, mbarrier: SYNCS, legacy tensor
-cores: HMMA, ldmatrix: LDSM, cp.async: LDGSTS, PDL: ACQBULK / PREEXIT ...).  Usage: python tools/sass_histogram.py [lib] > profiles/..."""
+a kernel uses (wgmma: HGMMA, TMA: UTMALDG / UBLKCP, mbarrier: SYNCS, legacy tensor
+cores: HMMA, ldmatrix: LDSM, cp.async: LDGSTS, PDL: ACQBULK / PREEXIT ...).  Usage: python tools/sass_histogram.py [lib] > <file>"""
 import collections
 import os
 import re
