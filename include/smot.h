@@ -32,7 +32,7 @@
 extern "C" {
 #endif
 
-#define SMOT_ABI_VERSION 4
+#define SMOT_ABI_VERSION 5
 
 enum { SMOT_OK = 0, SMOT_ERR_INVALID = 1, SMOT_ERR_CUDA = 2, SMOT_ERR_UNSUPPORTED = 3 };
 enum { SMOT_F32 = 0, SMOT_F16 = 1 };
@@ -127,6 +127,15 @@ typedef struct {
 int smot_roi_align(const smot_pyramid* pyr, const float* rois, const float* level_boxes, const int* count,
                    int max_rois, int channels, int res, int sampling_ratio, void* out, int dtype, void* stream);
 
+/* smot_roi_align_batched: the box-head pooling (box_head.py:46, through the upstream Pooler) of `batch` images of one size in
+ * one launch, for SiamMOT.forward on a (B,3,H,W) batch (rcnn.py:46-51 with the box head of roi_heads.py:25).  pyr describes
+ * image 0; level l of image b starts image_stride[l] elements (host array) after image b-1's.  rois: [batch][max_rois][4], image b's
+ * rows i < min(count[b], max_rois) are pooled from its own maps with smot_roi_align's in-kernel LevelMapper and arithmetic, the
+ * others are zero.  out: [batch][max_rois][res][res][C].  Each image's rows equal smot_roi_align on that image bit for bit.
+ * The ROIs choose their own level (no level_boxes); pyr->pad is honoured as in smot_roi_align. */
+int smot_roi_align_batched(const smot_pyramid* pyr, const long long* image_stride, int batch, const float* rois, const int* count,
+                           int max_rois, int channels, int res, int sampling_ratio, void* out, int dtype, void* stream);
+
 /* ---- RPN proposal selection (rpn_patch.py:15-60 + upstream select_over_all_levels) -------------
  * Per level: order anchors by objectness (descending, ties -> lower anchor index), take
  * pre_nms_top_n, decode with BoxCoder(1,1,1,1), clip unless amodal, drop boxes smaller than
@@ -144,6 +153,18 @@ int smot_rpn_select(const smot_rpn_level* levels, int num_levels, int pre_nms_to
                     float* out_boxes, float* out_scores, int* out_count, void* workspace, size_t workspace_bytes,
                     void* stream);
 
+/* smot_rpn_select_batched: smot_rpn_select for `batch` images of one size (the RPN inference of rcnn.py:48 over a (B,3,H,W)
+ * batch: upstream RPNPostProcessor.forward_for_single_feature_map per image + select_over_all_levels per image).  levels[l]
+ * describes image 0's head of level l; image b's starts head_image_stride[l] floats (host array) after image b-1's.  One launch
+ * sequence for all images (the image index is a grid dimension of every kernel).  Outputs out_boxes [batch][fpn_post_nms_top_n][4],
+ * out_scores [batch][fpn_post_nms_top_n], out_count [batch]; each image's result equals smot_rpn_select on that image alone bit
+ * for bit, (logit desc, anchor index asc) ties included.  The workspace is the single-image one per image. */
+size_t smot_rpn_select_batched_workspace(int num_levels, int pre_nms_top_n, int batch);
+int smot_rpn_select_batched(const smot_rpn_level* levels, const long long* head_image_stride, int batch, int num_levels,
+                            int pre_nms_top_n, int post_nms_top_n, float nms_thresh, float min_size, int fpn_post_nms_top_n,
+                            int img_w, int img_h, int amodal, float* out_boxes, float* out_scores, int* out_count, void* workspace,
+                            size_t workspace_bytes, void* stream);
+
 /* ---- sort + NMS (replaces _C.nms and the host-side mask reduction of upstream nms.cu) ----------
  * Rows i < min(n_max, *count) with scores[i*score_stride] > min_score are candidates.  They are
  * ordered by score descending (ties -> lower index), suppressed with IoU(+1) > thresh, and at most
@@ -156,6 +177,19 @@ int smot_sort_nms(const float* boxes, int box_stride, const float* scores, int s
                   float* out_scores, int* out_tag, int* out_count, void* workspace, size_t workspace_bytes,
                   void* stream);
 
+/* smot_sort_nms_segmented: the per-class NMS of the box head's filter_results (siammot/modelling/box_head/inference.py:145-191,
+ * boxlist_nms at :174) for `batch` images in one launch set, where the single-image path makes ncls-1 smot_sort_nms calls per image.
+ * boxes [batch][n_max][ncls][4] and scores [batch][n_max][ncls] are smot_box_decode's outputs per image.  Segment (b, j), j in
+ * [1, ncls): rows i < min(count[b], n_max) with scores > min_score, sorted, suppressed with IoU(+1) > thresh, at most max_keep kept
+ * -- smot_sort_nms on column j.  Image b's survivors go to its block: class j's behind class j-1's, each class in score order.
+ *   out_boxes [batch][cap][4], out_scores [batch][cap] (-1 past the image's count), out_block [batch][1 + cap] = count | labels.
+ * Each image's block equals what smot_sort_nms appends for classes 1 .. ncls-1 into a block whose scores were -1 and count 0.
+ * cap >= (ncls-1) * min(max_keep, n_max).  Kernels: sort, suppression mask, reduction, per-image scatter (4 launches). */
+size_t smot_sort_nms_segmented_workspace(int batch, int ncls, int n_max);
+int smot_sort_nms_segmented(const float* boxes, const float* scores, const int* count, int batch, int n_max, int ncls,
+                            float min_score, float thresh, int max_keep, int cap, float* out_boxes, float* out_scores,
+                            int* out_block, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- box head post-processing (inference.py:46-114 up to filter_results) ------------------------
  * head: fp32 [n_max][head_ld]: columns [0,ncls) class logits, [ncls + 4j + c] box deltas of class j.
  * For every row and class: softmax probability, BoxCoder(weights).decode, clip unless amodal.
@@ -165,6 +199,12 @@ int smot_sort_nms(const float* boxes, int box_stride, const float* scores, int s
 int smot_box_decode(const float* head, int head_ld, const float* rois, const int* count, int n_max, int ncls,
                     const float* weights4, int img_w, int img_h, int amodal, const int* track_labels,
                     float* out_boxes, float* out_scores, void* stream);
+/* smot_box_decode_batched: the same over `batch` segments of n_max rows (head [batch*n_max][head_ld], rois [batch][n_max][4],
+ * outputs [batch][n_max][ncls][4] / [batch][n_max][ncls]), segment b decoded against its own count[b]: rows at or past it get
+ * score -1 and a zero box, never a stale value.  No track rows.  Equal to smot_box_decode per image bit for bit. */
+int smot_box_decode_batched(const float* head, int head_ld, const float* rois, const int* count, int batch, int n_max, int ncls,
+                            const float* weights4, int img_w, int img_h, int amodal, float* out_boxes, float* out_scores,
+                            void* stream);
 
 /* ---- solver candidates: detections ++ refined tracks ---------------------------------------------
  * cat[0..ncap) = detections (as is); cat[ncap + r] = track r with its label's refined box and score

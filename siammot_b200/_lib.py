@@ -11,7 +11,7 @@ LIB_PATH = os.path.join(_HERE, "libsmot.so")
 F32, F16 = 0, 1
 CONV_AUTO, CONV_SIMT, CONV_TCGEN05 = 0, 1, 2
 MAX_LEVELS, MAX_ANCHORS = 5, 16
-ABI_VERSION = 4
+ABI_VERSION = 5
 CONV_WS_COUNTER_BYTES = 65536
 XCORR_ROW_PITCH, XCORR_PLANE = 40, 1208   # SMOT_XCORR_ROW_PITCH / SMOT_XCORR_PLANE: the channel-planar search-window layout
 
@@ -43,7 +43,8 @@ _lib = None
 KERNELS_PER_CALL = {"smot_conv2d": 1, "smot_image_to_nhwc": 1, "smot_maxpool2x2": 1, "smot_maxpool3x3s2": 1, "smot_deform_im2col3x3": 1, "smot_upsample_add": 1,
                     "smot_subsample2": 1, "smot_groupnorm_relu": 1, "smot_roi_align": 1, "smot_rpn_select": 6,
                     "smot_sort_nms": 3, "smot_box_decode": 1, "smot_track_combine": 1, "smot_track_combine_grouped": 1, "smot_xcorr": 1, "smot_emm_decode": 2,
-                    "smot_roi_align_planar": 1, "smot_xcorr_planar": 1, "smot_xcorr_planar_mode": 1, "smot_xcorr_planar_cfg": 1,
+                    "smot_roi_align_planar": 1, "smot_xcorr_planar": 1,
+                    "smot_roi_align_batched": 1, "smot_rpn_select_batched": 6, "smot_box_decode_batched": 1, "smot_sort_nms_segmented": 4, "smot_xcorr_planar_mode": 1, "smot_xcorr_planar_cfg": 1,
                     "smot_resample_h_u8": 1, "smot_resample_v_normalize": 1}
 
 
@@ -65,6 +66,10 @@ def _declare(lib):
         "smot_rpn_select": [C.POINTER(RpnLevel), i, i, i, f, f, i, i, i, i, vp, vp, vp, vp, sz, vp],
         "smot_sort_nms": [vp, i, vp, i, vp, i, f, f, i, i, vp, vp, vp, vp, vp, vp, sz, vp],
         "smot_box_decode": [vp, i, vp, vp, i, i, C.POINTER(C.c_float * 4), i, i, i, vp, vp, vp, vp],
+        "smot_roi_align_batched": [C.POINTER(Pyramid), vp, i, vp, vp, i, i, i, i, vp, i, vp],
+        "smot_rpn_select_batched": [C.POINTER(RpnLevel), vp, i, i, i, i, f, f, i, i, i, i, vp, vp, vp, vp, sz, vp],
+        "smot_box_decode_batched": [vp, i, vp, vp, i, i, i, C.POINTER(C.c_float * 4), i, i, i, vp, vp, vp],
+        "smot_sort_nms_segmented": [vp, vp, vp, i, i, i, f, f, i, i, vp, vp, vp, vp, sz, vp],
         "smot_track_combine": [vp, vp, i, vp, vp, i, vp, vp, vp, vp, i, i, vp, vp, vp, vp],
         "smot_track_combine_grouped": [vp, vp, i, vp, vp, i, vp, vp, vp, vp, i, i, vp, vp, vp, vp, vp],
         "smot_xcorr": [vp, vp, vp, i, i, i, i, i, vp],
@@ -85,6 +90,10 @@ def _declare(lib):
     lib.smot_rpn_select_workspace.restype = sz
     lib.smot_sort_nms_workspace.argtypes = [i]
     lib.smot_sort_nms_workspace.restype = sz
+    lib.smot_rpn_select_batched_workspace.argtypes = [i, i, i]
+    lib.smot_rpn_select_batched_workspace.restype = sz
+    lib.smot_sort_nms_segmented_workspace.argtypes = [i, i, i]
+    lib.smot_sort_nms_segmented_workspace.restype = sz
     lib.smot_resample_ksize.argtypes = [i, i]
     lib.smot_resample_ksize.restype = i
 

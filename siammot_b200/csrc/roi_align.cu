@@ -18,22 +18,28 @@ struct RoiArgs {
   smot_pyramid pyr;
   const float* rois;
   const float* level_boxes;
-  const int* count;
+  const int* count;      // [batch]
   int max_rois, channels, res, sampling;
+  // smot_roi_align_batched (the kernels' BATCHED instantiations): `batch` images, ROI row r belongs to image r / max_rois and
+  // samples level l of that image at pyr.feat[l] + image * img_stride[l] (elements); count[image] bounds the image's segment.
+  // The single-image instantiations never read these two fields, and compile to the code they had before batching existed.
+  int batch = 1;
+  long long img_stride[SMOT_MAX_LEVELS];
 };
 
-template <typename T>
+template <typename T, bool BATCHED = false>
 __global__ void roi_align_kernel(const RoiArgs a, T* __restrict__ out) {
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   const int bins = a.res * a.res;
-  if (warp >= a.max_rois * bins) return;
+  if (warp >= (BATCHED ? a.batch * a.max_rois : a.max_rois) * bins) return;
   const int r = warp / bins;
   const int bin = warp - r * bins;
   const int ph = bin / a.res, pw = bin - ph * a.res;
   T* dst = out + (size_t)warp * a.channels;
-  const int n = a.count ? min(*a.count, a.max_rois) : a.max_rois;
-  if (r >= n) {
+  const int img = BATCHED ? r / a.max_rois : 0;
+  const int n = a.count ? min(a.count[img], a.max_rois) : a.max_rois;
+  if (r - img * a.max_rois >= n) {
     for (int c = lane * 4; c < a.channels; c += 128) st4(dst + c, make_float4(0.f, 0.f, 0.f, 0.f));
     return;
   }
@@ -45,7 +51,7 @@ __global__ void roi_align_kernel(const RoiArgs a, T* __restrict__ out) {
   lv = fminf(fmaxf(lv, kmin), kmax);
   const int l = (int)lv - a.pyr.k_min;
 
-  const T* __restrict__ feat = reinterpret_cast<const T*>(a.pyr.feat[l]);
+  const T* __restrict__ feat = reinterpret_cast<const T*>(a.pyr.feat[l]) + (BATCHED ? img * a.img_stride[l] : 0);
   const int H = a.pyr.H[l], W = a.pyr.W[l], ld = a.pyr.ld[l], pad = a.pyr.pad[l];
   const int Hp = H + 2 * pad, Wp = W + 2 * pad;  // size of the (virtual) padded map
   const float sc = a.pyr.scale[l];
@@ -264,7 +270,7 @@ __device__ __forceinline__ float4 raw_to_f4(const Raw4<__half>& r) {
 // Round-2 instruction diet: ncu counted 818 warp instructions per bin (4 samples) in the previous form -- 64-bit index products
 // per corner, five-word table entries, per-corner predicates.  Now per sample: one 16-byte table load, 4 weight products, 4 adds +
 // 4 address computations + 4 loads, the conversions and the 32 multiply / add of the reference's summation order.
-template <typename T, bool PLANAR, int SAMP>
+template <typename T, bool PLANAR, int SAMP, bool BATCHED = false>
 __global__ void __launch_bounds__(256) roi_align_rows_kernel(const RoiArgs a, T* __restrict__ out, int row_pitch, int plane_pitch) {
   extern __shared__ __align__(16) unsigned char rar_raw[];
   __shared__ RarTap xs[RAR_MAX_SAMPLES];
@@ -276,8 +282,9 @@ __global__ void __launch_bounds__(256) roi_align_rows_kernel(const RoiArgs a, T*
   // that the roi's geometry and the sample tables are amortised over ~64+ bins even at 7 x 7)
   const int ph0 = PLANAR ? (int)blockIdx.x : (int)blockIdx.x * row_pitch, r = blockIdx.y;
   const int ph1 = PLANAR ? ph0 + 1 : min(a.res, ph0 + row_pitch);
-  const int n = a.count ? min(*a.count, a.max_rois) : a.max_rois;
-  if (r >= n) {   // rows past the count are zero
+  const int img = BATCHED ? r / a.max_rois : 0;   // the image of row r
+  const int n = a.count ? min(a.count[img], a.max_rois) : a.max_rois;
+  if (r - img * a.max_rois >= n) {   // rows past the image's count are zero
     if (PLANAR) {
       T* dst = out + (size_t)r * a.channels * plane_pitch + (size_t)ph0 * row_pitch;
       for (int i = threadIdx.x; i < a.channels * a.res; i += blockDim.x) {
@@ -297,7 +304,7 @@ __global__ void __launch_bounds__(256) roi_align_rows_kernel(const RoiArgs a, T*
   const float kmin = (float)a.pyr.k_min, kmax = (float)(a.pyr.k_min + a.pyr.num_levels - 1);
   lv = fminf(fmaxf(lv, kmin), kmax);
   const int l = (int)lv - a.pyr.k_min;
-  const T* __restrict__ feat = reinterpret_cast<const T*>(a.pyr.feat[l]);
+  const T* __restrict__ feat = reinterpret_cast<const T*>(a.pyr.feat[l]) + (BATCHED ? img * a.img_stride[l] : 0);
   const int H = a.pyr.H[l], W = a.pyr.W[l], ld = a.pyr.ld[l], pad = a.pyr.pad[l];
   const int Hp = H + 2 * pad, Wp = W + 2 * pad;
   const float sc = a.pyr.scale[l];
@@ -436,43 +443,70 @@ extern "C" int smot_roi_align_planar(const smot_pyramid* pyr, const float* rois,
   return SMOT_OK;
 }
 
-extern "C" int smot_roi_align(const smot_pyramid* pyr, const float* rois, const float* level_boxes, const int* count,
-                              int max_rois, int channels, int res, int sampling_ratio, void* out, int dtype,
-                              void* stream) {
-  SMOT_CHECK_ARG(pyr && out && (rois || max_rois == 0), "smot_roi_align: null argument");
-  SMOT_CHECK_ARG(pyr->num_levels >= 1 && pyr->num_levels <= SMOT_MAX_LEVELS, "smot_roi_align: num_levels %d", pyr->num_levels);
-  SMOT_CHECK_ARG(channels > 0 && channels % 4 == 0 && res > 0 && max_rois >= 0, "smot_roi_align: channels must be a multiple of 4");
+static int roi_align_nhwc(const char* who, const smot_pyramid* pyr, const long long* img_stride, int batch, const float* rois,
+                          const float* level_boxes, const int* count, int max_rois, int channels, int res, int sampling_ratio,
+                          void* out, int dtype, cudaStream_t st) {
+  SMOT_CHECK_ARG(pyr && out && (rois || max_rois == 0), "%s: null argument", who);
+  SMOT_CHECK_ARG(pyr->num_levels >= 1 && pyr->num_levels <= SMOT_MAX_LEVELS, "%s: num_levels %d", who, pyr->num_levels);
+  SMOT_CHECK_ARG(channels > 0 && channels % 4 == 0 && res > 0 && max_rois >= 0, "%s: channels must be a multiple of 4", who);
   for (int l = 0; l < pyr->num_levels; ++l)
     SMOT_CHECK_ARG(pyr->feat[l] && pyr->ld[l] % 4 == 0 && pyr->H[l] > 0 && pyr->W[l] > 0 && pyr->pad[l] >= 0,
-                   "smot_roi_align: bad level %d", l);
-  if (max_rois == 0) return SMOT_OK;
+                   "%s: bad level %d", who, l);
+  if (max_rois == 0 || batch == 0) return SMOT_OK;
   RoiArgs a;
   a.pyr = *pyr, a.rois = rois, a.level_boxes = level_boxes, a.count = count;
   a.max_rois = max_rois, a.channels = channels, a.res = res, a.sampling = sampling_ratio;
-  const long long warps = (long long)max_rois * res * res;
+  a.batch = batch;
+  for (int l = 0; l < SMOT_MAX_LEVELS; ++l) a.img_stride[l] = img_stride && l < pyr->num_levels ? img_stride[l] : 0;
+  const long long rows_total = (long long)batch * max_rois;
+  const long long warps = rows_total * res * res;
   const unsigned blocks = (unsigned)((warps * 32 + 255) / 256);
-  cudaStream_t st = (cudaStream_t)stream;
   const bool rows = roi_rows_enabled() && sampling_ratio > 0 && sampling_ratio <= 16 && res * sampling_ratio <= RAR_MAX_SAMPLES;
   // rows of bins per CTA: ~64+ bins, so that the per-CTA geometry + tables are amortised (7 x 7 -> the whole roi)
   int rpc = (64 + res - 1) / res;
   if (rpc > res) rpc = res;
   if (rpc * sampling_ratio > RAR_MAX_YS) rpc = RAR_MAX_YS / (sampling_ratio > 0 ? sampling_ratio : 1);
-  const dim3 grid((unsigned)((res + rpc - 1) / rpc), (unsigned)max_rois);
+  const dim3 grid((unsigned)((res + rpc - 1) / rpc), (unsigned)rows_total);
   const bool unroll = roi_unroll_enabled() && sampling_ratio == 2;
-  if (dtype == SMOT_F32 && rows && unroll)
-    roi_align_rows_kernel<float, false, 2><<<grid, 256, 0, st>>>(a, (float*)out, rpc, 0);
-  else if (dtype == SMOT_F16 && rows && unroll)
-    roi_align_rows_kernel<__half, false, 2><<<grid, 256, 0, st>>>(a, (__half*)out, rpc, 0);
-  else if (dtype == SMOT_F32 && rows)
-    roi_align_rows_kernel<float, false, 0><<<grid, 256, 0, st>>>(a, (float*)out, rpc, 0);
-  else if (dtype == SMOT_F16 && rows)
-    roi_align_rows_kernel<__half, false, 0><<<grid, 256, 0, st>>>(a, (__half*)out, rpc, 0);
-  else if (dtype == SMOT_F32)
-    roi_align_kernel<float><<<blocks, 256, 0, st>>>(a, (float*)out);
-  else if (dtype == SMOT_F16)
-    roi_align_kernel<__half><<<blocks, 256, 0, st>>>(a, (__half*)out);
-  else
-    SMOT_CHECK_ARG(false, "smot_roi_align: bad dtype %d", dtype);
-  SMOT_CHECK_LAUNCH("smot_roi_align");
+  const bool batched = img_stride != nullptr;   // smot_roi_align_batched: the BATCHED instantiations
+#define SMOT_ROI_LAUNCH(B_)                                                                                    \
+  if (dtype == SMOT_F32 && rows && unroll)                                                                     \
+    roi_align_rows_kernel<float, false, 2, B_><<<grid, 256, 0, st>>>(a, (float*)out, rpc, 0);                  \
+  else if (dtype == SMOT_F16 && rows && unroll)                                                                \
+    roi_align_rows_kernel<__half, false, 2, B_><<<grid, 256, 0, st>>>(a, (__half*)out, rpc, 0);                \
+  else if (dtype == SMOT_F32 && rows)                                                                          \
+    roi_align_rows_kernel<float, false, 0, B_><<<grid, 256, 0, st>>>(a, (float*)out, rpc, 0);                  \
+  else if (dtype == SMOT_F16 && rows)                                                                          \
+    roi_align_rows_kernel<__half, false, 0, B_><<<grid, 256, 0, st>>>(a, (__half*)out, rpc, 0);                \
+  else if (dtype == SMOT_F32)                                                                                  \
+    roi_align_kernel<float, B_><<<blocks, 256, 0, st>>>(a, (float*)out);                                       \
+  else if (dtype == SMOT_F16)                                                                                  \
+    roi_align_kernel<__half, B_><<<blocks, 256, 0, st>>>(a, (__half*)out);                                     \
+  else                                                                                                         \
+    SMOT_CHECK_ARG(false, "%s: bad dtype %d", who, dtype);
+  if (batched) {
+    SMOT_ROI_LAUNCH(true)
+  } else {
+    SMOT_ROI_LAUNCH(false)
+  }
+#undef SMOT_ROI_LAUNCH
+  SMOT_CHECK_LAUNCH(who);
   return SMOT_OK;
+}
+
+extern "C" int smot_roi_align(const smot_pyramid* pyr, const float* rois, const float* level_boxes, const int* count,
+                              int max_rois, int channels, int res, int sampling_ratio, void* out, int dtype,
+                              void* stream) {
+  return roi_align_nhwc("smot_roi_align", pyr, nullptr, 1, rois, level_boxes, count, max_rois, channels, res, sampling_ratio, out,
+                        dtype, (cudaStream_t)stream);
+}
+
+extern "C" int smot_roi_align_batched(const smot_pyramid* pyr, const long long* image_stride, int batch, const float* rois,
+                                      const int* count, int max_rois, int channels, int res, int sampling_ratio, void* out,
+                                      int dtype, void* stream) {
+  SMOT_CHECK_ARG(batch >= 0 && batch <= 65535 && image_stride && (count || batch <= 1),
+                 "smot_roi_align_batched: batch %d needs image strides and per-image counts", batch);
+  SMOT_CHECK_ARG((long long)batch * max_rois <= 65535, "smot_roi_align_batched: %d x %d rows exceed the grid", batch, max_rois);
+  return roi_align_nhwc("smot_roi_align_batched", pyr, image_stride, batch, rois, nullptr, count, max_rois, channels, res,
+                        sampling_ratio, out, dtype, (cudaStream_t)stream);
 }

@@ -52,7 +52,24 @@ struct SortNmsArgs {
   int words_max;
   // batching (blockIdx = problem): element offsets added per problem
   int in_step, out_step;
+  // segments (smot_sort_nms_segmented): seg > 0 classes per image; problem p is class p % seg of image p / seg, whose rows
+  // start at image * in_step rows + class * cls_*_step elements, bounded by count[image].  0: problem p is rows p * in_step...
+  int seg = 0, cls_box_step = 0, cls_score_step = 0;
 };
+
+// first box / score of problem `prob` and the index of its count.  SEG (compile time) = the segmented addressing; the other
+// instantiations are the unsegmented kernels as they were before segments existed.
+template <bool SEG> __device__ __forceinline__ int sn_image(const SortNmsArgs& a, int prob) { return SEG ? prob / a.seg : prob; }
+template <bool SEG> __device__ __forceinline__ const float* sn_boxes(const SortNmsArgs& a, int prob) {
+  if (!SEG) return a.boxes + (size_t)prob * a.in_step * a.box_stride;
+  const int img = prob / a.seg, cls = prob - img * a.seg;
+  return a.boxes + (size_t)img * a.in_step * a.box_stride + (size_t)cls * a.cls_box_step;
+}
+template <bool SEG> __device__ __forceinline__ const float* sn_scores(const SortNmsArgs& a, int prob) {
+  if (!SEG) return a.scores + (size_t)prob * a.in_step * a.score_stride;
+  const int img = prob / a.seg, cls = prob - img * a.seg;
+  return a.scores + (size_t)img * a.in_step * a.score_stride + (size_t)cls * a.cls_score_step;
+}
 
 // one compare-exchange pair per thread and stage
 __device__ __forceinline__ void bitonic_sort_desc(unsigned long long* keys, int np) {
@@ -73,15 +90,16 @@ __device__ __forceinline__ void bitonic_sort_desc(unsigned long long* keys, int 
 }
 
 // ---- K1: order the candidates -----------------------------------------------------------------
+template <bool SEG>
 __global__ void __launch_bounds__(SN_THREADS) nms_sort_kernel(SortNmsArgs a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   unsigned long long* keys = reinterpret_cast<unsigned long long*>(smem_raw);
   __shared__ int s_cnt;
   __shared__ int wcnt[SN_THREADS / 32];
   const int prob = blockIdx.x;
-  const float* boxes = a.boxes + (size_t)prob * a.in_step * a.box_stride;
-  const float* scores = a.scores + (size_t)prob * a.in_step * a.score_stride;
-  const int n = a.count ? min(a.count[prob], a.n_max) : a.n_max;
+  const float* boxes = sn_boxes<SEG>(a, prob);
+  const float* scores = sn_scores<SEG>(a, prob);
+  const int n = a.count ? min(a.count[sn_image<SEG>(a, prob)], a.n_max) : a.n_max;
   float4* sb = a.s_boxes + (size_t)prob * a.n_max;
   int* si = a.s_index + (size_t)prob * a.n_max;
   if (a.presorted) {
@@ -174,6 +192,7 @@ __global__ void __launch_bounds__(64) nms_mask_kernel(SortNmsArgs a) {
 }
 
 // ---- K3: greedy reduction + outputs ------------------------------------------------------------
+template <bool SEG>
 __global__ void __launch_bounds__(SN_THREADS) nms_reduce_kernel(SortNmsArgs a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   int* kept_all = reinterpret_cast<int*>(smem_raw);                                        // sorted row of the k-th survivor, [np]
@@ -184,7 +203,7 @@ __global__ void __launch_bounds__(SN_THREADS) nms_reduce_kernel(SortNmsArgs a) {
   __shared__ int s_kept, s_base, s_done;
   const int prob = blockIdx.x;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const float* scores = a.scores + (size_t)prob * a.in_step * a.score_stride;
+  const float* scores = sn_scores<SEG>(a, prob);
   const float4* __restrict__ sb = a.s_boxes + (size_t)prob * a.n_max;
   const int* __restrict__ si = a.s_index + (size_t)prob * a.n_max;
   const unsigned long long* gmask = a.mask + (size_t)prob * a.n_max * a.words_max;
@@ -307,11 +326,17 @@ static void carve_sort_nms_ws(SortNmsArgs& a, void* ws, int problems) {
 
 static int launch_sort_nms(SortNmsArgs& a, int problems, cudaStream_t st) {
   a.np = next_pow2(a.n_max);
-  SMOT_ENSURE_SMEM(nms_sort_kernel, SN_MAX * 8, "sort_nms(sort)");
-  SMOT_ENSURE_SMEM(nms_reduce_kernel, SN_MAX * 12 + SN_CACHE_BYTES, "sort_nms(reduce)");
+  SMOT_ENSURE_SMEM(nms_sort_kernel<false>, SN_MAX * 8, "sort_nms(sort)");
+  SMOT_ENSURE_SMEM(nms_reduce_kernel<false>, SN_MAX * 12 + SN_CACHE_BYTES, "sort_nms(reduce)");
+  SMOT_ENSURE_SMEM(nms_sort_kernel<true>, SN_MAX * 8, "sort_nms(sort)");
+  SMOT_ENSURE_SMEM(nms_reduce_kernel<true>, SN_MAX * 12 + SN_CACHE_BYTES, "sort_nms(reduce)");
+  const bool seg = a.seg > 0;
   // the bitonic network has np/2 compare-exchanges per stage: a smaller CTA makes its ~50 barriers cheaper
   const int sort_threads = a.presorted ? SN_THREADS : (a.np / 2 < 128 ? 128 : (a.np / 2 > SN_THREADS ? SN_THREADS : a.np / 2));
-  nms_sort_kernel<<<problems, sort_threads, a.presorted ? 0 : (size_t)a.np * 8, st>>>(a);
+  if (seg)
+    nms_sort_kernel<true><<<problems, sort_threads, a.presorted ? 0 : (size_t)a.np * 8, st>>>(a);
+  else
+    nms_sort_kernel<false><<<problems, sort_threads, a.presorted ? 0 : (size_t)a.np * 8, st>>>(a);
   SMOT_CHECK_LAUNCH("sort_nms(sort)");
   const bool suppress = a.thresh > 0.f && a.max_keep > 0;
   a.cache_pitch = 0;
@@ -323,7 +348,10 @@ static int launch_sort_nms(SortNmsArgs& a, int problems, cudaStream_t st) {
     const int pitch = a.words_max | 1;  // odd pitch: a column of 64-bit words spreads over all banks
     if ((size_t)a.n_max * pitch * 8 <= (size_t)SN_CACHE_BYTES) a.cache_pitch = pitch, cache_bytes = (size_t)a.n_max * pitch * 8;
   }
-  nms_reduce_kernel<<<problems, SN_THREADS, (size_t)a.np * 12 + cache_bytes, st>>>(a);
+  if (seg)
+    nms_reduce_kernel<true><<<problems, SN_THREADS, (size_t)a.np * 12 + cache_bytes, st>>>(a);
+  else
+    nms_reduce_kernel<false><<<problems, SN_THREADS, (size_t)a.np * 12 + cache_bytes, st>>>(a);
   SMOT_CHECK_LAUNCH("sort_nms(reduce)");
   return SMOT_OK;
 }
@@ -358,6 +386,9 @@ struct RpnArgs {
   float* out_boxes;
   float* out_scores;
   int* out_count;
+  // smot_rpn_select_batched (the kernels' BATCHED instantiations): image blockIdx.y reads its heads at lv[l].head + y *
+  // head_img_stride[l] and owns image slices of every array above ([image][...]).  Unread by smot_rpn_select's instantiations.
+  long long head_img_stride[SMOT_MAX_LEVELS];
 };
 
 // composite key: (objectness logit as monotone u32) << 22 | (2^22 - 1 - anchor index in the level): unique, and
@@ -445,6 +476,7 @@ __device__ void select_topk_u64(const unsigned long long* keys, int n, int k, un
   __syncthreads();
 }
 
+template <bool BATCHED>
 __global__ void __launch_bounds__(1024) rpn_local_topk_kernel(const RpnArgs a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   unsigned long long* keys = reinterpret_cast<unsigned long long*>(smem_raw);  // [RPN_CHUNK]
@@ -452,10 +484,11 @@ __global__ void __launch_bounds__(1024) rpn_local_topk_kernel(const RpnArgs a) {
   int lvl = 0;
   while (lvl + 1 < SMOT_MAX_LEVELS && (int)blockIdx.x >= a.chunk_first[lvl + 1]) ++lvl;
   const smot_rpn_level& L = a.lv[lvl];
+  const int img = BATCHED ? (int)blockIdx.y : 0;
   const int start = ((int)blockIdx.x - a.chunk_first[lvl]) * RPN_CHUNK;
   const int count = min(RPN_CHUNK, L.H * L.W * L.A - start);
   const int k = min(a.pre_nms_top_n, count);
-  const float* __restrict__ head = L.head;
+  const float* __restrict__ head = L.head + (BATCHED ? img * a.head_img_stride[lvl] : 0);
   const int A = L.A, ld = L.head_ld;
   for (int i = threadIdx.x; i < count; i += blockDim.x) {
     const int g = start + i;  // anchor index within the level: (cell * A + a)
@@ -463,20 +496,21 @@ __global__ void __launch_bounds__(1024) rpn_local_topk_kernel(const RpnArgs a) {
   }
   __syncthreads();
   select_topk_u64(keys, count, k, win);
-  unsigned long long* dst = a.local + (size_t)blockIdx.x * 1024;
+  unsigned long long* dst = a.local + ((size_t)img * a.nchunks + blockIdx.x) * 1024;
   for (int i = threadIdx.x; i < 1024; i += blockDim.x) dst[i] = win[i];
 }
 
+template <bool BATCHED>
 __global__ void __launch_bounds__(1024) rpn_merge_kernel(const RpnArgs a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   __shared__ unsigned long long cand[1024];
-  const int lvl = blockIdx.x;
+  const int lvl = blockIdx.x, img = BATCHED ? (int)blockIdx.y : 0;
   const smot_rpn_level& L = a.lv[lvl];
   const int c0 = a.chunk_first[lvl], c1 = a.chunk_first[lvl + 1];
   const int n = (c1 - c0) * 1024;
   const int total = L.H * L.W * L.A;
   const int k = min(a.pre_nms_top_n, total);
-  const unsigned long long* __restrict__ src = a.local + (size_t)c0 * 1024;
+  const unsigned long long* __restrict__ src = a.local + ((size_t)img * a.nchunks + c0) * 1024;
   if (c1 - c0 == 1) {
     for (int i = threadIdx.x; i < 1024; i += blockDim.x) cand[i] = src[i];
     __syncthreads();
@@ -490,9 +524,10 @@ __global__ void __launch_bounds__(1024) rpn_merge_kernel(const RpnArgs a) {
   }
   bitonic_sort_desc(cand, 1024);
   // ---- decode the k candidates in sorted order
-  const float* __restrict__ head = L.head;
-  float* cb = a.cand_boxes + (size_t)lvl * a.pre_nms_top_n * 4;
-  float* cs = a.cand_scores + (size_t)lvl * a.pre_nms_top_n;
+  const float* __restrict__ head = L.head + (BATCHED ? img * a.head_img_stride[lvl] : 0);
+  const int slot = img * a.num_levels + lvl;   // the (image, level) candidate slot
+  float* cb = a.cand_boxes + (size_t)slot * a.pre_nms_top_n * 4;
+  float* cs = a.cand_scores + (size_t)slot * a.pre_nms_top_n;
   for (int j = threadIdx.x; j < a.pre_nms_top_n; j += blockDim.x) {
     if (j >= k) {
       cs[j] = -1.f;
@@ -524,30 +559,37 @@ __global__ void __launch_bounds__(1024) rpn_merge_kernel(const RpnArgs a) {
     reinterpret_cast<float4*>(cb)[j] = make_float4(x1, y1, x2, y2);
     cs[j] = big ? score : -1.f;
   }
-  if (threadIdx.x == 0) a.cand_count[lvl] = k;
+  if (threadIdx.x == 0) a.cand_count[slot] = k;
 }
 
 // Cross-level top-n (upstream select_over_all_levels at test time: topk of the concatenated objectness).  Every
 // level's survivors are already in (score desc, position asc) order, so the global rank of a row is its own
 // position plus, per other level, the number of rows that precede it: rows of lower levels win ties (the order
 // topk sees in the level-major concatenation).  No sort, no CTA-wide synchronisation.
+template <bool BATCHED>
 __global__ void __launch_bounds__(256) rpn_final_kernel(const RpnArgs a) {
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   const int P = a.post_nms_top_n;
+  const int img = BATCHED ? (int)blockIdx.y : 0;   // this image's slices of the kept arrays and of the outputs
+  const int* kept_count = a.kept_count + (size_t)img * a.num_levels;
+  const float* kept_scores = a.kept_scores + (size_t)img * a.num_levels * P;
+  const float* kept_boxes = a.kept_boxes + (size_t)img * a.num_levels * P * 4;
+  float* out_boxes = a.out_boxes + (size_t)img * a.final_top_n * 4;
+  float* out_scores = a.out_scores + (size_t)img * a.final_top_n;
   if (e == 0) {
     int total = 0;
-    for (int l = 0; l < a.num_levels; ++l) total += min(a.kept_count[l], P);
-    *a.out_count = min(total, a.final_top_n);
+    for (int l = 0; l < a.num_levels; ++l) total += min(kept_count[l], P);
+    a.out_count[img] = min(total, a.final_top_n);
   }
   if (e >= a.num_levels * P) return;
   const int l = e / P, p = e - l * P;
-  if (p >= min(a.kept_count[l], P)) return;
-  const float s = a.kept_scores[e];
+  if (p >= min(kept_count[l], P)) return;
+  const float s = kept_scores[e];
   int rank = p;
   for (int o = 0; o < a.num_levels; ++o) {
     if (o == l) continue;
-    const float* so = a.kept_scores + (size_t)o * P;
-    int lo = 0, hi = min(a.kept_count[o], P);  // first position in level o that does NOT precede (l, p)
+    const float* so = kept_scores + (size_t)o * P;
+    int lo = 0, hi = min(kept_count[o], P);  // first position in level o that does NOT precede (l, p)
     while (lo < hi) {
       const int mid = (lo + hi) >> 1;
       const float v = so[mid];
@@ -556,22 +598,26 @@ __global__ void __launch_bounds__(256) rpn_final_kernel(const RpnArgs a) {
     rank += lo;
   }
   if (rank < a.final_top_n) {
-    reinterpret_cast<float4*>(a.out_boxes)[rank] = reinterpret_cast<const float4*>(a.kept_boxes)[e];
-    a.out_scores[rank] = s;
+    reinterpret_cast<float4*>(out_boxes)[rank] = reinterpret_cast<const float4*>(kept_boxes)[e];
+    out_scores[rank] = s;
   }
 }
 
 // ---------------------------------------------------------------------------------------------
 // box head: softmax + per-class decode
 // ---------------------------------------------------------------------------------------------
+// BATCHED (smot_box_decode_batched): rows are `batch` segments of n_max, row r is row r % n_max of image r / n_max and is decoded
+// only below count[image]; the rest of a segment gets score -1 and an empty box, so no later step can read a stale row.
+template <bool BATCHED>
 __global__ void box_decode_kernel(const float* __restrict__ head, int head_ld, const float* __restrict__ rois,
-                                  const int* count, int n_max, int ncls, float wx, float wy, float ww, float wh,
+                                  const int* count, int n_max, int batch, int ncls, float wx, float wy, float ww, float wh,
                                   int img_w, int img_h, int amodal, const int* track_labels,
                                   float* __restrict__ out_boxes, float* __restrict__ out_scores) {
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= n_max) return;
-  const int n = count ? min(*count, n_max) : n_max;
-  if (r >= n) {
+  if (r >= (BATCHED ? batch * n_max : n_max)) return;
+  const int img = BATCHED ? r / n_max : 0;
+  const int n = count ? min(count[img], n_max) : n_max;
+  if (r - img * n_max >= n) {
     for (int j = 0; j < ncls; ++j) {
       out_scores[(size_t)r * ncls + j] = -1.f;
       reinterpret_cast<float4*>(out_boxes)[(size_t)r * ncls + j] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -603,6 +649,43 @@ __global__ void box_decode_kernel(const float* __restrict__ head, int head_ld, c
     }
     out_scores[(size_t)r * ncls + j] = prob;
     reinterpret_cast<float4*>(out_boxes)[(size_t)r * ncls + j] = make_float4(x1, y1, x2, y2);
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
+// per-image detection blocks of the segmented per-class NMS (smot_sort_nms_segmented)
+// ---------------------------------------------------------------------------------------------
+// One CTA per (image, class) segment.  The NMS kernels left segment p's survivors as original row indices, in kept order, in
+// kept_index[p][0 .. kept_n[p]).  The per-class loop of the single-image path appends class j's survivors behind those of
+// classes 1 .. j-1, so a segment's first output row is the prefix sum of the keep counts of the image's lower classes: every
+// CTA recomputes that prefix (ncls - 1 loads) and scatters its rows; the image's class-1 CTA writes the count and marks the
+// rest of the block invalid (score -1), which is what the loop's fill + appends leave behind.
+__global__ void __launch_bounds__(256) nms_scatter_segments_kernel(const float* __restrict__ boxes, const float* __restrict__ scores,
+                                                                   int n_max, int ncls, const int* __restrict__ kept_index,
+                                                                   const int* __restrict__ kept_n, int cap, float* __restrict__ out_boxes,
+                                                                   float* __restrict__ out_scores, int* __restrict__ out_block) {
+  const int K = ncls - 1;
+  const int prob = blockIdx.x, img = prob / K, cls = prob - img * K;
+  int base = 0, total = 0;
+  for (int q = 0; q < K; ++q) {
+    const int c = kept_n ? kept_n[img * K + q] : 0;
+    total += c;
+    base += q < cls ? c : 0;
+  }
+  const int m = kept_n ? kept_n[prob] : 0;   // (null: no candidates at all)
+  const int* idx = kept_index + (size_t)prob * n_max;
+  float* ob = out_boxes + (size_t)img * cap * 4;
+  float* os = out_scores + (size_t)img * cap;
+  int* blk = out_block + (size_t)img * (1 + cap);
+  for (int k = threadIdx.x; k < m; k += blockDim.x) {
+    const size_t row = ((size_t)img * n_max + idx[k]) * ncls + cls + 1;
+    reinterpret_cast<float4*>(ob)[base + k] = reinterpret_cast<const float4*>(boxes)[row];
+    os[base + k] = scores[row];
+    blk[1 + base + k] = cls + 1;
+  }
+  if (cls == 0) {
+    for (int k = total + threadIdx.x; k < cap; k += blockDim.x) os[k] = -1.f;
+    if (threadIdx.x == 0) blk[0] = total;
   }
 }
 
@@ -748,40 +831,51 @@ static int rpn_chunk_count(const smot_rpn_level* levels, int num_levels) {
   return n;
 }
 
-extern "C" size_t smot_rpn_select_workspace(int num_levels, int pre_nms_top_n) {
-  if (num_levels <= 0 || pre_nms_top_n <= 0) return 0;
-  const size_t L = (size_t)num_levels, P = (size_t)pre_nms_top_n;
+static size_t rpn_ws_bytes(int num_levels, int pre_nms_top_n, int batch) {
+  const size_t L = (size_t)num_levels * batch, P = (size_t)pre_nms_top_n;   // L = (image, level) slots
   size_t b = 0;
-  b += align256(L * P * 16);                         // cand_boxes
-  b += align256(L * P * 4);                          // cand_scores
-  b += align256(L * 4);                              // cand_count
-  b += align256(L * P * 16);                         // kept boxes per level
-  b += align256(L * P * 4);                          // kept scores per level
-  b += align256(L * 4);                              // kept count per level
-  b += align256((size_t)RPN_MAX_CHUNKS * 1024 * 8);  // local winners
-  b += sort_nms_ws_bytes(num_levels, pre_nms_top_n); // per-level NMS
+  b += align256(L * P * 16);                                 // cand_boxes
+  b += align256(L * P * 4);                                  // cand_scores
+  b += align256(L * 4);                                      // cand_count
+  b += align256(L * P * 16);                                 // kept boxes per level
+  b += align256(L * P * 4);                                  // kept scores per level
+  b += align256(L * 4);                                      // kept count per level
+  b += align256((size_t)batch * RPN_MAX_CHUNKS * 1024 * 8);  // local winners
+  b += sort_nms_ws_bytes((int)L, pre_nms_top_n);             // per-level NMS
   return b;
 }
 
-extern "C" int smot_rpn_select(const smot_rpn_level* levels, int num_levels, int pre_nms_top_n, int post_nms_top_n,
-                               float nms_thresh, float min_size, int fpn_post_nms_top_n, int img_w, int img_h,
-                               int amodal, float* out_boxes, float* out_scores, int* out_count, void* workspace,
-                               size_t workspace_bytes, void* stream) {
-  SMOT_CHECK_ARG(levels && out_boxes && out_scores && out_count && workspace, "smot_rpn_select: null argument");
-  SMOT_CHECK_ARG(num_levels >= 1 && num_levels <= SMOT_MAX_LEVELS, "smot_rpn_select: num_levels %d", num_levels);
-  SMOT_CHECK_ARG(pre_nms_top_n >= 1 && pre_nms_top_n <= 1024, "smot_rpn_select: pre_nms_top_n %d not in [1,1024]", pre_nms_top_n);
-  SMOT_CHECK_ARG(post_nms_top_n >= 1 && post_nms_top_n <= pre_nms_top_n, "smot_rpn_select: post_nms_top_n %d", post_nms_top_n);
-  SMOT_CHECK_ARG(num_levels * post_nms_top_n <= SN_MAX, "smot_rpn_select: levels*post_nms_top_n > %d", SN_MAX);
-  SMOT_CHECK_ARG(workspace_bytes >= smot_rpn_select_workspace(num_levels, pre_nms_top_n), "smot_rpn_select: workspace too small");
+extern "C" size_t smot_rpn_select_workspace(int num_levels, int pre_nms_top_n) {
+  if (num_levels <= 0 || pre_nms_top_n <= 0) return 0;
+  return rpn_ws_bytes(num_levels, pre_nms_top_n, 1);
+}
+
+extern "C" size_t smot_rpn_select_batched_workspace(int num_levels, int pre_nms_top_n, int batch) {
+  if (num_levels <= 0 || pre_nms_top_n <= 0 || batch <= 0) return 0;
+  return rpn_ws_bytes(num_levels, pre_nms_top_n, batch);
+}
+
+// smot_rpn_select over `batch` images: every kernel's grid has the image in y (the per-level NMS: problem = image * levels +
+// level), so the launch sequence is the single-image one and each image's arithmetic is the single-image arithmetic.
+static int rpn_select(const char* who, const smot_rpn_level* levels, const long long* head_img_stride, int batch, int num_levels,
+                      int pre_nms_top_n, int post_nms_top_n, float nms_thresh, float min_size, int fpn_post_nms_top_n, int img_w,
+                      int img_h, int amodal, float* out_boxes, float* out_scores, int* out_count, void* workspace,
+                      size_t workspace_bytes, cudaStream_t st) {
+  SMOT_CHECK_ARG(levels && out_boxes && out_scores && out_count && workspace, "%s: null argument", who);
+  SMOT_CHECK_ARG(batch >= 1 && batch <= 1024, "%s: batch %d", who, batch);
+  SMOT_CHECK_ARG(num_levels >= 1 && num_levels <= SMOT_MAX_LEVELS, "%s: num_levels %d", who, num_levels);
+  SMOT_CHECK_ARG(pre_nms_top_n >= 1 && pre_nms_top_n <= 1024, "%s: pre_nms_top_n %d not in [1,1024]", who, pre_nms_top_n);
+  SMOT_CHECK_ARG(post_nms_top_n >= 1 && post_nms_top_n <= pre_nms_top_n, "%s: post_nms_top_n %d", who, post_nms_top_n);
+  SMOT_CHECK_ARG(num_levels * post_nms_top_n <= SN_MAX, "%s: levels*post_nms_top_n > %d", who, SN_MAX);
+  SMOT_CHECK_ARG(workspace_bytes >= rpn_ws_bytes(num_levels, pre_nms_top_n, batch), "%s: workspace too small", who);
   for (int l = 0; l < num_levels; ++l)
     SMOT_CHECK_ARG(levels[l].head && levels[l].A >= 1 && levels[l].A <= SMOT_MAX_ANCHORS && levels[l].H > 0 && levels[l].W > 0 &&
                        levels[l].head_ld >= 5 * levels[l].A &&
                        (long long)levels[l].H * levels[l].W * levels[l].A <= (long long)RPN_IDX_MASK,
-                   "smot_rpn_select: bad level %d", l);
+                   "%s: bad level %d", who, l);
   const int nchunks = rpn_chunk_count(levels, num_levels);
-  SMOT_CHECK_ARG(nchunks <= RPN_MAX_CHUNKS, "smot_rpn_select: feature maps too large (%d chunks > %d)", nchunks, RPN_MAX_CHUNKS);
-  cudaStream_t st = (cudaStream_t)stream;
-  const size_t L = (size_t)num_levels, P = (size_t)pre_nms_top_n;
+  SMOT_CHECK_ARG(nchunks <= RPN_MAX_CHUNKS, "%s: feature maps too large (%d chunks > %d)", who, nchunks, RPN_MAX_CHUNKS);
+  const size_t L = (size_t)num_levels * batch, P = (size_t)pre_nms_top_n;
   unsigned char* w = (unsigned char*)workspace;
   float* cand_boxes = (float*)w;   w += align256(L * P * 16);
   float* cand_scores = (float*)w;  w += align256(L * P * 4);
@@ -789,13 +883,14 @@ extern "C" int smot_rpn_select(const smot_rpn_level* levels, int num_levels, int
   float* kept_boxes = (float*)w;   w += align256(L * P * 16);
   float* kept_scores = (float*)w;  w += align256(L * P * 4);
   int* kept_count = (int*)w;       w += align256(L * 4);
-  unsigned long long* local = (unsigned long long*)w; w += align256((size_t)RPN_MAX_CHUNKS * 1024 * 8);
+  unsigned long long* local = (unsigned long long*)w; w += align256((size_t)batch * RPN_MAX_CHUNKS * 1024 * 8);
   void* ws_level = w;
 
   RpnArgs ra;
   int nc = 0, widest = 0;
   for (int l = 0; l < SMOT_MAX_LEVELS; ++l) {
     ra.chunk_first[l] = nc;
+    ra.head_img_stride[l] = head_img_stride && l < num_levels ? head_img_stride[l] : 0;
     if (l < num_levels) {
       ra.lv[l] = levels[l];
       const int c = (levels[l].H * levels[l].W * levels[l].A + RPN_CHUNK - 1) / RPN_CHUNK;
@@ -812,11 +907,23 @@ extern "C" int smot_rpn_select(const smot_rpn_level* levels, int num_levels, int
   ra.cand_boxes = cand_boxes, ra.cand_scores = cand_scores, ra.cand_count = cand_count;
   ra.kept_boxes = kept_boxes, ra.kept_scores = kept_scores, ra.kept_count = kept_count;
   ra.out_boxes = out_boxes, ra.out_scores = out_scores, ra.out_count = out_count;
-  SMOT_ENSURE_SMEM(rpn_local_topk_kernel, RPN_CHUNK * 8, "smot_rpn_select(local top-k)");
-  SMOT_ENSURE_SMEM(rpn_merge_kernel, RPN_MERGE_SMEM_KEYS * 8, "smot_rpn_select(merge)");
-  rpn_local_topk_kernel<<<nc, 1024, RPN_CHUNK * 8, st>>>(ra);
+  // the batched entry point takes the BATCHED instantiations; smot_rpn_select the ones without image offsets
+  const bool batched = head_img_stride != nullptr;
+  const size_t merge_smem = ra.merge_in_smem && widest > 1 ? (size_t)widest * 1024 * 8 : 0;
+  if (batched) {
+    SMOT_ENSURE_SMEM(rpn_local_topk_kernel<true>, RPN_CHUNK * 8, "smot_rpn_select(local top-k)");
+    SMOT_ENSURE_SMEM(rpn_merge_kernel<true>, RPN_MERGE_SMEM_KEYS * 8, "smot_rpn_select(merge)");
+    rpn_local_topk_kernel<true><<<dim3(nc, batch), 1024, RPN_CHUNK * 8, st>>>(ra);
+  } else {
+    SMOT_ENSURE_SMEM(rpn_local_topk_kernel<false>, RPN_CHUNK * 8, "smot_rpn_select(local top-k)");
+    SMOT_ENSURE_SMEM(rpn_merge_kernel<false>, RPN_MERGE_SMEM_KEYS * 8, "smot_rpn_select(merge)");
+    rpn_local_topk_kernel<false><<<nc, 1024, RPN_CHUNK * 8, st>>>(ra);
+  }
   SMOT_CHECK_LAUNCH("smot_rpn_select(local top-k)");
-  rpn_merge_kernel<<<num_levels, 1024, ra.merge_in_smem && widest > 1 ? (size_t)widest * 1024 * 8 : 0, st>>>(ra);
+  if (batched)
+    rpn_merge_kernel<true><<<dim3(num_levels, batch), 1024, merge_smem, st>>>(ra);
+  else
+    rpn_merge_kernel<false><<<num_levels, 1024, merge_smem, st>>>(ra);
   SMOT_CHECK_LAUNCH("smot_rpn_select(merge)");
 
   // per-level NMS (the candidates are already in score order), survivors into slots of post_nms_top_n rows
@@ -826,14 +933,36 @@ extern "C" int smot_rpn_select(const smot_rpn_level* levels, int num_levels, int
   a.append = 0, a.fill_tail = post_nms_top_n, a.presorted = 1;
   a.out_index = nullptr, a.out_boxes = kept_boxes, a.out_scores = kept_scores, a.out_tag = nullptr, a.out_count = kept_count;
   a.in_step = pre_nms_top_n, a.out_step = post_nms_top_n;
-  carve_sort_nms_ws(a, ws_level, num_levels);
-  int rc = launch_sort_nms(a, num_levels, st);
+  carve_sort_nms_ws(a, ws_level, (int)L);
+  int rc = launch_sort_nms(a, (int)L, st);
   if (rc) return rc;
 
   // cross-level top-n
-  rpn_final_kernel<<<(num_levels * post_nms_top_n + 255) / 256, 256, 0, st>>>(ra);
+  if (batched)
+    rpn_final_kernel<true><<<dim3((num_levels * post_nms_top_n + 255) / 256, batch), 256, 0, st>>>(ra);
+  else
+    rpn_final_kernel<false><<<(num_levels * post_nms_top_n + 255) / 256, 256, 0, st>>>(ra);
   SMOT_CHECK_LAUNCH("smot_rpn_select(final)");
   return SMOT_OK;
+}
+
+extern "C" int smot_rpn_select(const smot_rpn_level* levels, int num_levels, int pre_nms_top_n, int post_nms_top_n,
+                               float nms_thresh, float min_size, int fpn_post_nms_top_n, int img_w, int img_h,
+                               int amodal, float* out_boxes, float* out_scores, int* out_count, void* workspace,
+                               size_t workspace_bytes, void* stream) {
+  return rpn_select("smot_rpn_select", levels, nullptr, 1, num_levels, pre_nms_top_n, post_nms_top_n, nms_thresh, min_size,
+                    fpn_post_nms_top_n, img_w, img_h, amodal, out_boxes, out_scores, out_count, workspace, workspace_bytes,
+                    (cudaStream_t)stream);
+}
+
+extern "C" int smot_rpn_select_batched(const smot_rpn_level* levels, const long long* head_image_stride, int batch, int num_levels,
+                                       int pre_nms_top_n, int post_nms_top_n, float nms_thresh, float min_size,
+                                       int fpn_post_nms_top_n, int img_w, int img_h, int amodal, float* out_boxes,
+                                       float* out_scores, int* out_count, void* workspace, size_t workspace_bytes, void* stream) {
+  SMOT_CHECK_ARG(head_image_stride, "smot_rpn_select_batched: null head_image_stride");
+  return rpn_select("smot_rpn_select_batched", levels, head_image_stride, batch, num_levels, pre_nms_top_n, post_nms_top_n,
+                    nms_thresh, min_size, fpn_post_nms_top_n, img_w, img_h, amodal, out_boxes, out_scores, out_count, workspace,
+                    workspace_bytes, (cudaStream_t)stream);
 }
 
 extern "C" int smot_box_decode(const float* head, int head_ld, const float* rois, const int* count, int n_max, int ncls,
@@ -842,9 +971,74 @@ extern "C" int smot_box_decode(const float* head, int head_ld, const float* rois
   SMOT_CHECK_ARG(n_max >= 0 && ncls >= 2 && head_ld >= 5 * ncls && weights4, "smot_box_decode: bad arguments");
   if (n_max == 0) return SMOT_OK;
   SMOT_CHECK_ARG(head && rois && out_boxes && out_scores, "smot_box_decode: null argument");
-  box_decode_kernel<<<(n_max + 127) / 128, 128, 0, (cudaStream_t)stream>>>(
-      head, head_ld, rois, count, n_max, ncls, weights4[0], weights4[1], weights4[2], weights4[3], img_w, img_h, amodal,
+  box_decode_kernel<false><<<(n_max + 127) / 128, 128, 0, (cudaStream_t)stream>>>(
+      head, head_ld, rois, count, n_max, 1, ncls, weights4[0], weights4[1], weights4[2], weights4[3], img_w, img_h, amodal,
       track_labels, out_boxes, out_scores);
   SMOT_CHECK_LAUNCH("smot_box_decode");
+  return SMOT_OK;
+}
+
+extern "C" int smot_box_decode_batched(const float* head, int head_ld, const float* rois, const int* count, int batch, int n_max,
+                                       int ncls, const float* weights4, int img_w, int img_h, int amodal, float* out_boxes,
+                                       float* out_scores, void* stream) {
+  SMOT_CHECK_ARG(batch >= 0 && n_max >= 0 && ncls >= 2 && head_ld >= 5 * ncls && weights4 && count,
+                 "smot_box_decode_batched: bad arguments");
+  const long long rows = (long long)batch * n_max;
+  if (rows == 0) return SMOT_OK;
+  SMOT_CHECK_ARG(rows <= (1ll << 30), "smot_box_decode_batched: %lld rows", rows);
+  SMOT_CHECK_ARG(head && rois && out_boxes && out_scores, "smot_box_decode_batched: null argument");
+  box_decode_kernel<true><<<(unsigned)((rows + 127) / 128), 128, 0, (cudaStream_t)stream>>>(
+      head, head_ld, rois, count, n_max, batch, ncls, weights4[0], weights4[1], weights4[2], weights4[3], img_w, img_h, amodal,
+      nullptr, out_boxes, out_scores);
+  SMOT_CHECK_LAUNCH("smot_box_decode_batched");
+  return SMOT_OK;
+}
+
+static size_t segmented_ws_bytes(int problems, int n_max) {
+  return sort_nms_ws_bytes(problems, n_max) + align256((size_t)problems * n_max * 4) + align256((size_t)problems * 4);
+}
+
+extern "C" size_t smot_sort_nms_segmented_workspace(int batch, int ncls, int n_max) {
+  if (batch <= 0 || ncls < 2 || n_max <= 0) return 0;
+  return segmented_ws_bytes(batch * (ncls - 1), n_max);
+}
+
+extern "C" int smot_sort_nms_segmented(const float* boxes, const float* scores, const int* count, int batch, int n_max, int ncls,
+                                       float min_score, float thresh, int max_keep, int cap, float* out_boxes, float* out_scores,
+                                       int* out_block, void* workspace, size_t workspace_bytes, void* stream) {
+  SMOT_CHECK_ARG(batch >= 0 && ncls >= 2 && n_max >= 0 && n_max <= SN_MAX && max_keep >= 0,
+                 "smot_sort_nms_segmented: bad arguments (batch %d, ncls %d, n_max %d)", batch, ncls, n_max);
+  if (batch == 0) return SMOT_OK;
+  const int K = ncls - 1, problems = batch * K;
+  SMOT_CHECK_ARG(problems <= 65535, "smot_sort_nms_segmented: %d segments", problems);
+  SMOT_CHECK_ARG(boxes && scores && count && out_boxes && out_scores && out_block, "smot_sort_nms_segmented: null argument");
+  SMOT_CHECK_ARG((long long)cap >= (long long)K * (max_keep < n_max ? max_keep : n_max),
+                 "smot_sort_nms_segmented: cap %d < %d classes x %d survivors", cap, K, max_keep < n_max ? max_keep : n_max);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (n_max == 0) {   // no candidates: every image's block is empty
+    nms_scatter_segments_kernel<<<problems, 256, 0, st>>>(boxes, scores, 0, ncls, nullptr, nullptr, cap, out_boxes, out_scores,
+                                                          out_block);
+    SMOT_CHECK_LAUNCH("smot_sort_nms_segmented(scatter)");
+    return SMOT_OK;
+  }
+  SMOT_CHECK_ARG(workspace && workspace_bytes >= segmented_ws_bytes(problems, n_max),
+                 "smot_sort_nms_segmented: workspace too small (%zu < %zu)", workspace_bytes, segmented_ws_bytes(problems, n_max));
+  unsigned char* w = (unsigned char*)workspace + sort_nms_ws_bytes(problems, n_max);
+  int* kept_index = (int*)w;
+  int* kept_n = (int*)(w + align256((size_t)problems * n_max * 4));
+  // the single-image NMS kernels over all (image, class) segments; survivors stay in the workspace as row indices
+  SortNmsArgs a;
+  a.boxes = boxes + 4, a.box_stride = 4 * ncls, a.scores = scores + 1, a.score_stride = ncls, a.count = count;   // class 1 on
+  a.n_max = n_max, a.min_score = min_score, a.thresh = thresh, a.max_keep = max_keep, a.tag = 0;
+  a.append = 0, a.fill_tail = 0, a.presorted = 0;
+  a.out_index = kept_index, a.out_boxes = nullptr, a.out_scores = nullptr, a.out_tag = nullptr, a.out_count = kept_n;
+  a.in_step = n_max, a.out_step = n_max;
+  a.seg = K, a.cls_box_step = 4, a.cls_score_step = 1;
+  carve_sort_nms_ws(a, workspace, problems);
+  int rc = launch_sort_nms(a, problems, st);
+  if (rc) return rc;
+  nms_scatter_segments_kernel<<<problems, 256, 0, st>>>(boxes, scores, n_max, ncls, kept_index, kept_n, cap, out_boxes, out_scores,
+                                                        out_block);
+  SMOT_CHECK_LAUNCH("smot_sort_nms_segmented(scatter)");
   return SMOT_OK;
 }

@@ -148,6 +148,8 @@ class _Plan(object):
         self.part_graphs = [None, None]
         self.branch = None            # while building: steps appended go to this parallel branch (None = main line)
         self.batch = 1                # images per backbone pass (2 = a frame PAIR of a clip, see Engine.pair_plan)
+        self.batched = False          # Engine.batch_plan: the detection tail runs over all `batch` images too
+        self.branch_wss = None        # split-K scratch per parallel branch when the plan owns them (batch plans)
         self.bufs = []                # activation buffers in allocation order
         self.view_of, self.view_index, self._cursor = None, 0, 0
 
@@ -176,7 +178,12 @@ class _Plan(object):
 
     def conv(self, x, name, out, residual=None, stride=1, pad=0, relu=False):
         w, scale, bias = self.e.weights[name]
-        ws = self.ws if self.branch is None else self.e.branch_ws(self.branch, getattr(self, "slot", 0))
+        if self.branch is None:
+            ws = self.ws
+        elif self.branch_wss is not None:
+            ws = self.branch_wss[self.branch]
+        else:
+            ws = self.e.branch_ws(self.branch, getattr(self, "slot", 0))
         d = ops.conv_desc(x, w, out, scale, bias, residual, stride, pad, relu, workspace=ws)
         self.keep.append(d)
         self.steps.append((lib().smot_conv2d, (C.byref(d),), "conv:" + name, self.branch))
@@ -954,6 +961,45 @@ class Engine(object):
         self.plans[key] = PP
         return PP
 
+    def batch_plan(self, H, W, B):
+        """Static plan of the whole frame-independent stage (backbone, FPN, RPN heads, proposal selection, box head, per-class
+        NMS) over B images of one size as ONE launch list, captured as a CUDA graph like the per-frame plans; cached per
+        (H, W, B).  The detection tail uses the batched entry points (smot_rpn_select_batched, smot_roi_align_batched,
+        smot_box_decode_batched, smot_sort_nms_segmented) and the box-head GEMMs run as B images of 1 x nprop rows, so every
+        image's detections equal those of plan(H, W) on that image bit for bit.  Outputs: det_boxes (B, cap, 4), det_scores
+        (B, cap), det_block (B, 1 + cap) = count | labels.  B = 1 is plan(H, W)."""
+        if B < 2:
+            raise ValueError("batch_plan is for B >= 2 images (B = 1 runs on Engine.plan)")
+        key = (H, W, "batch", B)
+        if key in self.plans:
+            return self.plans[key]
+        self._check_plan_size(H, W)
+        P = _Plan(self, H, W)
+        P.batch = B
+        P.batched = True
+        P.slot = ("batch", B)
+        # Split-K scratch scaled to B images.  A layer's split factor depends on one image's tiles, but it is taken only when
+        # the partial tiles of the whole batch fit the scratch: B times the single-image room keeps every split decision, and
+        # with it the fp32 summation order, equal to the B = 1 plan's.
+        nbytes = _lib.CONV_WS_COUNTER_BYTES + B * (self.conv_ws.numel() - _lib.CONV_WS_COUNTER_BYTES)
+        P.ws = ops.conv_workspace(self.device, nbytes)
+        P.branch_wss = [ops.conv_workspace(self.device, nbytes) for _ in range(4)]
+        P.det_ws = ops.conv_workspace(self.device, _lib.CONV_WS_COUNTER_BYTES + B * (self.conv_ws_det.numel()
+                                                                                      - _lib.CONV_WS_COUNTER_BYTES))
+        P.keep += [P.ws, P.det_ws] + P.branch_wss
+        self._build_static(P)
+        self.plans[key] = P
+        return P
+
+    def run_batch(self, images):
+        """images: (B, 3, H, W) float tensor (any device), B >= 2.  Enqueues batch_plan(H, W, B) on the current stream."""
+        B, _, H, W = images.shape
+        P = self.batch_plan(H, W, B)
+        P.img_batch.copy_(images, non_blocking=True)
+        with self.timed("static"):
+            P.run()
+        return P
+
     def _check_plan_size(self, H, W):
         if not self.weights:
             raise RuntimeError("Engine.load_state_dict() must be called before the first frame")
@@ -1030,6 +1076,8 @@ class Engine(object):
         P.feats = feats
         if backbone_only:
             return
+        if P.batched:
+            return self._batched_tail(P, heads, feats)
         if P.batch != 1:
             raise RuntimeError("the detection tail runs per frame: build it on a frame plan (Engine.pair_plan(...).frames[i])")
         # ---- RPN selection
@@ -1066,6 +1114,62 @@ class Engine(object):
                                      nprop, H_.SCORE_THRESH, H_.NMS, nprop, j, None, ops._ptr(P.det_boxes),
                                      ops._ptr(P.det_scores), ops._ptr(P.det_labels), ops._ptr(P.det_count), ops._ptr(nws),
                                      nws.numel()), "det_nms%d" % j)
+
+    def _batched_tail(self, P, heads, feats):
+        """The detection tail of a batch plan: the per-frame tail's steps over P.batch images, each step one launch set."""
+        cfg, dev, L = self.cfg, self.device, lib()
+        B, H, W = P.batch, P.H, P.W
+        R, Hh, H_ = cfg.MODEL.RPN, cfg.MODEL.ROI_BOX_HEAD, cfg.MODEL.ROI_HEADS
+        ncls, res = self.ncls, Hh.POOLER_RESOLUTION
+        # ---- RPN selection, all images
+        P.rpn_levels = ops.rpn_levels(heads, R.ANCHOR_STRIDE, self.cells)
+        head_strides = ops.image_strides(heads)
+        nprop = R.FPN_POST_NMS_TOP_N_TEST
+        P.props = torch.zeros((B, nprop, 4), dtype=torch.float32, device=dev)
+        P.prop_scores = torch.zeros((B, nprop), dtype=torch.float32, device=dev)
+        P.prop_count = torch.zeros((B,), dtype=torch.int32, device=dev)
+        ws = ops.rpn_select_batched_workspace(len(feats), R.PRE_NMS_TOP_N_TEST, B, dev)
+        P.keep += [P.rpn_levels, head_strides, ws]
+        P.call(L.smot_rpn_select_batched, (P.rpn_levels, head_strides, B, len(feats), R.PRE_NMS_TOP_N_TEST, R.POST_NMS_TOP_N_TEST,
+                                           R.NMS_THRESH, float(R.MIN_SIZE), nprop, W, H, int(cfg.INPUT.AMODAL), ops._ptr(P.props),
+                                           ops._ptr(P.prop_scores), ops._ptr(P.prop_count), ops._ptr(ws), ws.numel()), "rpn_select")
+        # ---- box head: ROIAlign over B segments of nprop rows, then fc6 / fc7 / predictor as B images of 1 x nprop rows (the
+        # split-K factor is chosen per image, so each image's sums run in the B = 1 order)
+        P.ws = P.det_ws
+        rep = Hh.MLP_HEAD_DIM
+        hld = ((5 * ncls + 3) // 4) * 4
+        dt = self.dtype
+        box = P.box = dict(pooled=torch.zeros((B * nprop, res, res, self.C), dtype=dt, device=dev),
+                           fc6=torch.zeros((B, 1, nprop, rep), dtype=dt, device=dev),
+                           fc7=torch.zeros((B, 1, nprop, rep), dtype=dt, device=dev),
+                           head=torch.zeros((B, 1, nprop, hld), dtype=torch.float32, device=dev),
+                           dec_boxes=torch.zeros((B * nprop, ncls, 4), dtype=torch.float32, device=dev),
+                           dec_scores=torch.zeros((B * nprop, ncls), dtype=torch.float32, device=dev), n=nprop)
+        pyr = ops.make_pyramid(feats, Hh.POOLER_SCALES)
+        feat_strides = ops.image_strides(feats[:len(Hh.POOLER_SCALES)])
+        P.keep += [pyr, feat_strides]
+        P.call(L.smot_roi_align_batched, (C.byref(pyr), feat_strides, B, ops._ptr(P.props), ops._ptr(P.prop_count), nprop, self.C,
+                                          res, Hh.POOLER_SAMPLING_RATIO, ops._ptr(box["pooled"]), _lib.dtype_code(dt)), "box_roi_align")
+        P.conv(box["pooled"].view(B, 1, nprop, res * res * self.C), "box.fc6", box["fc6"], relu=True)
+        P.conv(box["fc6"], "box.fc7", box["fc7"], relu=True)
+        P.conv(box["fc7"], "box.pred", box["head"][..., :5 * ncls])
+        w4 = (C.c_float * 4)(*[float(w) for w in H_.BBOX_REG_WEIGHTS])
+        P.keep.append(w4)
+        P.call(L.smot_box_decode_batched, (ops._ptr(box["head"]), hld, ops._ptr(P.props), ops._ptr(P.prop_count), B, nprop, ncls,
+                                           C.byref(w4), W, H, int(cfg.INPUT.AMODAL), ops._ptr(box["dec_boxes"]),
+                                           ops._ptr(box["dec_scores"])), "box_decode")
+        # ---- per-class NMS of every (image, class) segment into per-image blocks
+        cap = nprop * (ncls - 1)
+        # boxes | scores | [count | labels] of all images in ONE buffer: the batch's results leave in one copy
+        P.det_packed = torch.zeros((B * (6 * cap + 1),), dtype=torch.float32, device=dev)
+        P.det_boxes = P.det_packed[:B * cap * 4].view(B, cap, 4)
+        P.det_scores = P.det_packed[B * cap * 4:B * cap * 5].view(B, cap)
+        P.det_block = P.det_packed[B * cap * 5:].view(torch.int32).view(B, 1 + cap)
+        nws = ops.sort_nms_segmented_workspace(B, ncls, nprop, dev)
+        P.keep.append(nws)
+        P.call(L.smot_sort_nms_segmented, (ops._ptr(box["dec_boxes"]), ops._ptr(box["dec_scores"]), ops._ptr(P.prop_count), B, nprop,
+                                           ncls, H_.SCORE_THRESH, H_.NMS, nprop, cap, ops._ptr(P.det_boxes), ops._ptr(P.det_scores),
+                                           ops._ptr(P.det_block), ops._ptr(nws), nws.numel()), "det_nms")
 
     def _fill_dets(self, P):
         P.det_scores.fill_(-1.0)

@@ -314,6 +314,63 @@ class CombinedROIHeads(nn.ModuleDict):
         ids = np.full((k,), -1, dtype=np.int64)                         # inference.py:90: detections carry id -1
         return self._to_boxlist(boxes, scores, ids, labels, (P.W, P.H)), None
 
+    # -- MODEL.TRACK_ON False over a (B,3,H,W) batch (rcnn.py:46-51 with roi_heads.py:25; inferencer.py:60 with CLIP_LEN > 1)
+    def detections_batch(self, P):
+        """B BoxLists, in image order, from the result blocks of batch plan P (enqueued on the current stream): one packed
+        device-to-host copy and one host wait for the whole batch."""
+        B, cap = P.det_scores.shape
+        host = getattr(P, "det_host", None)
+        if host is None:
+            host = P.det_host = torch.zeros((P.det_packed.numel(),), dtype=torch.float32).pin_memory()
+            P.det_done = torch.cuda.Event()
+        host.copy_(P.det_packed, non_blocking=True)
+        P.det_done.record()
+        P.det_done.synchronize()
+        h = host.numpy()
+        boxes = h[:B * cap * 4].reshape(B, cap, 4)
+        scores = h[B * cap * 4:B * cap * 5].reshape(B, cap)
+        blk = h[B * cap * 5:].view(np.int32).reshape(B, 1 + cap)
+        items = []
+        for b in range(B):
+            k = int(blk[b, 0])
+            items.append((np.array(boxes[b, :k], dtype=np.float32, copy=True), np.array(scores[b, :k], dtype=np.float32, copy=True),
+                          np.full((k,), -1, dtype=np.int64), blk[b, 1:1 + k].astype(np.int64)))   # inference.py:90: ids -1
+        return self._to_boxlists(items, (P.W, P.H), P)
+
+    def _to_boxlists(self, items, size, P):
+        """_to_boxlist for a batch: with results on the device, ONE packed pinned block and one host-to-device copy for all
+        images (the BoxList fields are views of it); the block is per plan and reused once its previous copy has completed."""
+        if self.results_on_host:
+            return [self._to_boxlist(bx, sc, ids, lab, size) for bx, sc, ids, lab in items]
+        ks = [bx.shape[0] for bx, _, _, _ in items]
+        spans = [(36 * k + 7) & ~7 for k in ks]   # each image's fields start 8-byte aligned (int64 views)
+        nbytes = sum(spans)
+        stage = getattr(P, "out_stage", None)
+        if stage is not None:
+            stage[1].synchronize()
+        if stage is None or stage[0].numel() < nbytes:
+            stage = P.out_stage = [torch.zeros((max(nbytes, 36 * 256),), dtype=torch.uint8).pin_memory(), torch.cuda.Event()]
+        h = stage[0].numpy()
+        offs, o = [], 0
+        for (bx, sc, ids, lab), k, span in zip(items, ks, spans):
+            h[o:o + 8 * k].view(np.int64)[:] = ids
+            h[o + 8 * k:o + 16 * k].view(np.int64)[:] = lab
+            h[o + 16 * k:o + 32 * k].view(np.float32)[:] = bx.reshape(-1)
+            h[o + 32 * k:o + 36 * k].view(np.float32)[:] = sc
+            offs.append(o)
+            o += span
+        d = torch.empty((max(nbytes, 8),), dtype=torch.uint8, device=self.engine.device)
+        d[:nbytes].copy_(stage[0][:nbytes], non_blocking=True)
+        stage[1].record()
+        out = []
+        for o, k in zip(offs, ks):
+            r = BoxList(d[o + 16 * k:o + 32 * k].view(torch.float32).view(k, 4), size, mode="xyxy")
+            r.add_field("scores", d[o + 32 * k:o + 36 * k].view(torch.float32))
+            r.add_field("ids", d[o:o + 8 * k].view(torch.int64))
+            r.add_field("labels", d[o + 8 * k:o + 16 * k].view(torch.int64))
+            out.append(r)
+        return out
+
     def finish_frame(self, pending, next_P=None, defer=None, before_solver=None):
         """Wait for the frame's result block, resolve ids on the host, build the next-frame memory.
         next_P: the static plan the NEXT frame will run on (clip pipelining); defaults to this frame's.
@@ -615,8 +672,11 @@ class SiamMOT(nn.Module):
         if self.training:
             raise NotImplementedError("siammot_b200 is an inference engine: call .eval() (training is out of scope)")
         eng = self.engine()
+        sizes = getattr(images, "image_sizes", None)
         if hasattr(images, "tensors"):
             images = images.tensors
+        if torch.is_tensor(images) and images.dim() == 4 and images.shape[0] > 1 and images.dtype != torch.uint8:
+            return self._forward_batch(eng, images, sizes, given_detection)
         mem_in = self._mem
         overlap = (eng.frame_overlap and given_detection is None and self.cfg.MODEL.TRACK_ON and mem_in is not None
                    and mem_in.feat is not None and mem_in.feat.numel() > 0)
@@ -634,6 +694,28 @@ class SiamMOT(nn.Module):
         self._mem = mem
         self.track_memory = mem
         return [result]
+
+
+def _forward_batch(self, eng, images, sizes, given_detection):
+    """A (B,3,H,W) batch, B >= 2, through a detector-only model: Engine.batch_plan runs the frame-independent stage of all B
+    images as one launch list; returns B BoxLists in image order, each equal to model(images[i:i+1])[0]."""
+    B, _, H, W = images.shape
+    if self.cfg.MODEL.TRACK_ON:
+        raise ValueError("a tracking model (MODEL.TRACK_ON True) takes one image per forward, as the reference's EMM asserts "
+                         "(track_core.py:75); got a batch of %d" % B)
+    if given_detection is not None:
+        raise ValueError("given_detection is supported for one image per forward only; got a batch of %d images" % B)
+    if sizes is not None and any(tuple(int(v) for v in sz) != (H, W) for sz in sizes):
+        raise ValueError("padded ImageList: image_sizes %s differ from the batch tensor's %dx%d; a batch must hold images of one "
+                         "size" % ([tuple(int(v) for v in sz) for sz in sizes], H, W))
+    P = eng.run_batch(images)
+    result = self.roi_heads.detections_batch(P)
+    self._mem = None
+    self.track_memory = None
+    return result
+
+
+SiamMOT._forward_batch = _forward_batch
 
 
 def _forward_overlapped(self, eng, P, mem):

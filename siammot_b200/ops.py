@@ -322,3 +322,74 @@ def emm_decode(maps, sr, tboxes, hann, up, T, pad, use_centerness, sigma, img_w,
                                 int(use_centerness), float(sigma), img_w, img_h, int(amodal), _ptr(boxes), _ptr(conf),
                                 _ptr(valid), _ptr(scratch), stream_ptr()), "smot_emm_decode")
     return boxes, conf, valid
+
+
+# ---- batched detection stage (B images of one size; Engine.batch_plan) ------------------------------------------------------
+def image_strides(maps):
+    """Host array of the per-image element strides of NHWC maps (B, H, W, C): what the batched entry points add per image."""
+    arr = (C.c_longlong * _lib.MAX_LEVELS)()
+    for l, m in enumerate(maps):
+        B, H, W, _, ld = _nhwc(m)
+        arr[l] = H * W * ld
+    return arr
+
+
+def rpn_select_batched_workspace(num_levels, pre_nms_top_n, batch, device):
+    nbytes = lib().smot_rpn_select_batched_workspace(num_levels, pre_nms_top_n, batch)
+    return torch.empty((nbytes,), dtype=torch.uint8, device=device)
+
+
+def sort_nms_segmented_workspace(batch, ncls, n_max, device):
+    return torch.empty((max(lib().smot_sort_nms_segmented_workspace(batch, ncls, n_max), 8),), dtype=torch.uint8, device=device)
+
+
+def rpn_select_batched(heads, levels, pre_nms_top_n, post_nms_top_n, nms_thresh, min_size, fpn_post_nms_top_n, img_w, img_h,
+                       amodal, out_boxes, out_scores, out_count, workspace):
+    """heads: the (B,H,W,ld) fp32 head maps ``levels`` (rpn_levels) describes; outputs (B,n,4), (B,n), (B,) int32."""
+    _require_cuda(out_boxes, out_scores, out_count, *heads)
+    strides = image_strides(heads)
+    check(lib().smot_rpn_select_batched(levels, strides, heads[0].shape[0], len(levels), pre_nms_top_n, post_nms_top_n, nms_thresh,
+                                        float(min_size), fpn_post_nms_top_n, img_w, img_h, int(amodal), _ptr(out_boxes),
+                                        _ptr(out_scores), _ptr(out_count), _ptr(workspace),
+                                        workspace.numel() * workspace.element_size(), stream_ptr()), "smot_rpn_select_batched")
+
+
+def roi_align_batched(feats, rois, count, scales, res, sampling, out=None):
+    """feats: (B,H,W,C) level maps; rois (B,n,4) fp32, count (B,) int32 -> (B*n, res, res, C)."""
+    _require_cuda(rois, count, *feats)
+    B, n = rois.shape[0], rois.shape[1]
+    Cc = feats[0].shape[3]
+    if out is None:
+        out = torch.empty((B * n, res, res, Cc), dtype=feats[0].dtype, device=feats[0].device)
+    p = make_pyramid(feats, scales)
+    assert rois.dtype == torch.float32 and rois.is_contiguous() and count.dtype == torch.int32
+    check(lib().smot_roi_align_batched(C.byref(p), image_strides(feats), B, _ptr(rois), _ptr(count), n, Cc, res, sampling, _ptr(out),
+                                       dtype_code(feats[0].dtype), stream_ptr()), "smot_roi_align_batched")
+    return out
+
+
+def box_decode_batched(head, rois, count, ncls, weights, img_w, img_h, amodal, out_boxes=None, out_scores=None):
+    """head: fp32 (B*n, ld); rois (B,n,4); count (B,) -> boxes (B*n, ncls, 4), scores (B*n, ncls)."""
+    _require_cuda(head, rois, count)
+    B, n = rois.shape[0], rois.shape[1]
+    if out_boxes is None:
+        out_boxes = torch.empty((B * n, ncls, 4), dtype=torch.float32, device=head.device)
+        out_scores = torch.empty((B * n, ncls), dtype=torch.float32, device=head.device)
+    w4 = (C.c_float * 4)(*[float(w) for w in weights])
+    check(lib().smot_box_decode_batched(_ptr(head), head.stride(0), _ptr(rois), _ptr(count), B, n, ncls, C.byref(w4), img_w, img_h,
+                                        int(amodal), _ptr(out_boxes), _ptr(out_scores), stream_ptr()), "smot_box_decode_batched")
+    return out_boxes, out_scores
+
+
+def sort_nms_segmented(boxes, scores, count, batch, ncls, min_score, thresh, max_keep, out_boxes, out_scores, out_block,
+                       workspace=None):
+    """boxes (B*n, ncls, 4), scores (B*n, ncls), count (B,) -> per-image blocks out_boxes (B,cap,4), out_scores (B,cap),
+    out_block (B,1+cap) = count | labels.  See smot.h."""
+    _require_cuda(boxes, scores, count, out_boxes, out_scores, out_block)
+    n = boxes.shape[0] // batch
+    cap = out_scores.shape[1]
+    if workspace is None:
+        workspace = sort_nms_segmented_workspace(batch, ncls, n, boxes.device)
+    check(lib().smot_sort_nms_segmented(_ptr(boxes), _ptr(scores), _ptr(count), batch, n, ncls, min_score, thresh, max_keep, cap,
+                                        _ptr(out_boxes), _ptr(out_scores), _ptr(out_block), _ptr(workspace), workspace.numel(),
+                                        stream_ptr()), "smot_sort_nms_segmented")
