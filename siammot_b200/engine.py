@@ -22,8 +22,6 @@ a few single-element glue ops on tiny tensors.  No CPU fallback exists.
 import ctypes as C
 import math
 import os
-import queue
-import threading
 
 import torch
 
@@ -63,36 +61,6 @@ def cell_anchors(stride, sizes, aspect_ratios):
         w, h, xc, yc = whctr(ra)
         rows.append(mk(w * scales, h * scales, xc, yc))
     return torch.from_numpy(np.vstack(rows)).float()
-
-
-class _Enqueuer(threading.Thread):
-    """Daemon thread that runs the clip pipeline's enqueue jobs in submission order.  A job is a callable; `done` (a
-    threading.Event) is set when it has run.  An exception is kept and re-raised on the submitting thread by check()."""
-
-    def __init__(self):
-        super().__init__(name="smot-enqueue", daemon=True)
-        self.q = queue.SimpleQueue()
-        self.error = None
-
-    def run(self):
-        while True:
-            fn, done = self.q.get()
-            try:
-                if fn is not None and self.error is None:
-                    fn()
-            except BaseException as exc:   # noqa: B902 -- handed to the caller's thread
-                self.error = exc
-            finally:
-                if done is not None:
-                    done.set()
-
-    def submit(self, fn, done=None):
-        self.q.put((fn, done))
-
-    def check(self):
-        if self.error is not None:
-            exc, self.error = self.error, None
-            raise exc
 
 
 class _NoTimer(object):
@@ -183,7 +151,7 @@ class _Plan(object):
         elif self.branch_wss is not None:
             ws = self.branch_wss[self.branch]
         else:
-            ws = self.e.branch_ws(self.branch, getattr(self, "slot", 0))
+            ws = self.e.branch_ws(self.branch)
         d = ops.conv_desc(x, w, out, scale, bias, residual, stride, pad, relu, workspace=ws)
         self.keep.append(d)
         self.steps.append((lib().smot_conv2d, (C.byref(d),), "conv:" + name, self.branch))
@@ -584,42 +552,23 @@ class Engine(object):
         self.conv_ws_det = ops.conv_workspace(self.device)
         self._side = None
         self._tail = None
-        # developer switches of SiamMOT.forward_clip (DESIGN.md section 4): SMOT_CLIP_SPLIT=1 runs the detection tail of frame t
-        # on a third stream under the backbone of frame t+1; SMOT_CLIP_SLOTS = number of static-plan copies (2 or 3)
-        self.body_branches = os.environ.get("SMOT_BODY_BRANCHES", "0") == "1"
         # SiamMOT.forward: detection tail of the frame on a second stream under the EMM half of its track stage
         # (default; identical tracks; =0 restores the serial order)
         self.frame_overlap = os.environ.get("SMOT_FRAME_OVERLAP", "1") == "1"
-        # forward_clip: three-stage pipeline over 3 static-plan copies by default (round 2: measured 989 / 1071 FPS value / e2e
-        # faster than the two-stream pipeline on earlier hardware, identical tracks); SMOT_CLIP_SPLIT=0 = two-stream
+        # forward_clip (DESIGN.md section 4): SMOT_CLIP_SPLIT=1 (default) is the three-stage pipeline, which runs the detection
+        # tail of frame t on a third stream under the backbone of frame t+1 (round 2: measured 989 / 1071 FPS value / e2e faster
+        # than the two-stream pipeline on earlier hardware, identical tracks); SMOT_CLIP_SPLIT=0 = two-stream.
+        # SMOT_CLIP_SLOTS = number of static-plan copies of the three-stage pipeline (2 to 4, default 3)
         self.clip_split = os.environ.get("SMOT_CLIP_SPLIT", "1") == "1"
         self.clip_slots = max(2, min(4, int(os.environ.get("SMOT_CLIP_SLOTS", "3"))))
-        self._pre = None
-        self._branch_ws = {}
-        self._slot_ws = {}
-        self._bb_streams = []
-        # forward_clip (three-stage): number of streams the backbone halves of consecutive frames alternate over (needs
-        # SMOT_CLIP_SLOTS >= streams + 1 plan copies to matter)
-        self.clip_backbone_streams = max(1, min(3, int(os.environ.get("SMOT_CLIP_BACKBONE_STREAMS", "1"))))
         # forward_clip (three-stage): backbone half over frame pairs (Engine.pair_plan); SMOT_CLIP_PAIRS=0 = one frame per pass
         self.clip_pairs = os.environ.get("SMOT_CLIP_PAIRS", "1") == "1"
-        # forward_clip: the host work nothing waits for (result BoxList, per-id cache update) runs under the NEXT frame's track
-        # stage instead of in front of it (SMOT_CLIP_DEFER=0: in line, as model(frame) does)
-        self.clip_defer = os.environ.get("SMOT_CLIP_DEFER", "1") == "1"
-        # forward_clip (three-stage): the backbone / detection-tail enqueues (graph launches, input copies) and the deferred
-        # host work run on a helper thread, so the caller's thread only carries the sequential chain of a video
-        # (track stage launch -> wait -> solver -> next memory).  SMOT_CLIP_THREAD=0: everything on the caller's thread.
-        # Measured slower and noisier on earlier hardware -- the clip is bound by the GPU
-        # (backbone + detection tail + track stage co-scheduled: 0.86 ms per frame), the time the caller's thread saves only
-        # moves into its wait for the track stage, and two Python threads contend for the GIL.  Off by default.
-        self.clip_thread = os.environ.get("SMOT_CLIP_THREAD", "0") == "1"
-        self._enqueuer = None
-        self.clip_thread_force = False   # tests: use the helper thread although the launch lists are not CUDA graphs
+        self._pre = None
+        self._branch_ws = {}
         self._branch_streams = []
         self._track_plans = {}
         self._arenas = {}
-        # developer switch (DESIGN.md section 9): exchange the EMM search windows channel-planar (smot_roi_align_planar ->
-        # smot_xcorr_planar).  Off by default until it has been through the GPU tests.
+        # SMOT_NVTX=1: NVTX ranges around the stages (see timed())
         self.nvtx = os.environ.get("SMOT_NVTX", "0") == "1"
         # channel-planar search-window exchange (default since round 2: bit-equal windows, 1.5-2x faster correlation on the
         # earlier hardware); 0 = NHWC windows + xcorr_mma_kernel, 1 = planar with the untrimmed MMA phase, 2 = trimmed (libsmot reads it)
@@ -730,66 +679,15 @@ class Engine(object):
     # ------------------------------------------------------------------------------------------
     # static plan
     # ------------------------------------------------------------------------------------------
-    def _tree(self, P, name, x, levels, cin, cout, stride, level_root, out=None, rootbuf=None):
-        """DlaTree (dla.py:192-238) as launches.  x / out are NHWC views.  Returns the output view."""
-        _, H, W, _ = x.shape
-        Ho, Wo = H // stride, W // stride
-        if levels == 1:
-            total = 2 * cout + (cin if level_root else 0)
-            if rootbuf is None:
-                rootbuf = P.new(Ho, Wo, total)
-            else:
-                assert not level_root
-            x2v, x1v = rootbuf[..., 0:cout], rootbuf[..., cout:2 * cout]
-            # developer switch SMOT_BODY_BRANCHES=1: the residual path (max-pool -> 1x1 project) and tree1.conv1 both read x and
-            # nothing of each other -- as two branches of the graph the two small kernels run under the 3x3 conv
-            side = self.body_branches and stride > 1 and cin != cout and P.branch is None
-            if side:
-                P.fork(1)
-                P.branch = 0
-            if stride > 1:
-                bottom = rootbuf[..., 2 * cout:2 * cout + cin] if level_root else P.new(Ho, Wo, cin)
-                P.call(lib().smot_maxpool2x2, self._pool_args(x, bottom), "maxpool:" + name)
-            else:
-                bottom = x
-            if cin != cout:
-                residual = P.new(Ho, Wo, cout)
-                P.conv(bottom, "body." + name + ".project.0", residual)
-            else:
-                residual = bottom
-            if side:
-                P.branch = None
-            a = P.new(Ho, Wo, cout)
-            P.conv(x, "body." + name + ".tree1.conv1", a, stride=stride, pad=1, relu=True)
-            if side:
-                P.join()
-            P.conv(a, "body." + name + ".tree1.conv2", x1v, residual=residual, pad=1, relu=True)
-            b = P.new(Ho, Wo, cout)
-            P.conv(x1v, "body." + name + ".tree2.conv1", b, pad=1, relu=True)
-            P.conv(b, "body." + name + ".tree2.conv2", x2v, residual=x1v, pad=1, relu=True)
-            if out is None:
-                out = P.new(Ho, Wo, cout)
-            P.conv(rootbuf, "body." + name + ".root.conv", out, relu=True)
-            return out
-        assert levels == 2, "DLA-34 only nests two tree levels"
-        total = 2 * cout + (cin if level_root else 0) + cout
-        rootbuf = P.new(Ho, Wo, total)
-        off = 2 * cout
-        if level_root:
-            P.call(lib().smot_maxpool2x2, self._pool_args(x, rootbuf[..., off:off + cin]), "maxpool:" + name)
-            off += cin
-        # the outer project (dla.py:228 overwrites its result) is dead code: skipped, results identical
-        t1 = rootbuf[..., off:off + cout]
-        self._tree(P, name + ".tree1", x, 1, cin, cout, stride, False, out=t1)
-        return self._tree(P, name + ".tree2", t1, 1, cout, cout, 1, False, out=out, rootbuf=rootbuf)
-
     def _tree_general(self, P, name, x, levels, cin, cout, stride, level_root, bottleneck, root_residual, out=None, rootbuf=None,
                       off=None, with_dcn=False):
-        """DlaTree of any depth with either block type (the DLA family beyond DLA-34: dla.py:316-372), concat-free.
+        """DlaTree (dla.py:192-238) of any depth with either block type (every DLA body, dla.py:307-372) as launches,
+        concat-free.  x / out are NHWC views; returns the output view.
         The innermost tree2 of a nest owns the root (dla.py:209-210); its input [x2 | x1 | bottom? | x1 of every enclosing
         tree, outermost first] (dla.py:229-237) is ONE buffer allocated where the nest starts: every producer writes its
         channel slice in place.  ``rootbuf`` / ``off``: that buffer and its next free channel when this call is the tree2 chain
-        of an enclosing tree.  As in _tree, the ``project`` of a tree whose tree1 is itself a tree is dead code (dla.py:228)."""
+        of an enclosing tree.  The ``project`` of a tree whose tree1 is itself a tree is dead code (dla.py:228 overwrites its
+        result): skipped, results identical."""
         _, H, W, _ = x.shape
         Ho, Wo = H // stride, W // stride
         if rootbuf is None:
@@ -849,7 +747,7 @@ class Engine(object):
         return out
 
     def _dla_body_general(self, P, img):
-        """DLA.forward (dla.py:289-304) for the family members other than DLA-34 (whose hand-laid plan is _tree)."""
+        """DLA.forward (dla.py:289-304) for every member of the DLA family (synthetic.DLA_ARCHS), DLA-34 included."""
         from .synthetic import DLA_ARCHS
         A = DLA_ARCHS[self.cfg.MODEL.BACKBONE.CONV_BODY]
         ch, lv = A["channels"], A["levels"]
@@ -923,7 +821,6 @@ class Engine(object):
         self._check_plan_size(H, W)
         P = _Plan(self, H, W)
         P.slot = slot
-        P.ws = self.backbone_ws(slot)
         self._build_static(P)
         self.plans[key] = P
         return P
@@ -1022,21 +919,7 @@ class Engine(object):
         P.img_in = P.img_batch[0]
         img = P.new(H, W, 4)
         P.per_image(L.smot_image_to_nhwc, lambda i: (ops._ptr(P.img_batch[i]), ops._ptr(img[i:i + 1]), 3, H, W, 4, dc), "image_to_nhwc")
-        if self.resnet:
-            body = self._resnet_body(P, img)
-        elif cfg.MODEL.BACKBONE.CONV_BODY != "DLA-34-FPN":
-            body = self._dla_body_general(P, img)
-        else:
-            # ---- DLA-34 body (dla.py:289-304)
-            ch = (16, 32, 64, 128, 256, 512)
-            x = P.conv(img[..., :3], "body.base_layer.0", P.new(H, W, ch[0]), pad=3, relu=True)
-            x = P.conv(x, "body.level0.0", P.new(H, W, ch[0]), pad=1, relu=True)
-            x = P.conv(x, "body.level1.0", P.new(H // 2, W // 2, ch[1]), stride=2, pad=1, relu=True)
-            x2 = self._tree(P, "level2", x, 1, ch[1], ch[2], 2, False)
-            x3 = self._tree(P, "level3", x2, 2, ch[2], ch[3], 2, True)
-            x4 = self._tree(P, "level4", x3, 2, ch[3], ch[4], 2, True)
-            x5 = self._tree(P, "level5", x4, 1, ch[4], ch[5], 2, True)
-            body = [x2, x3, x4, x5]
+        body = self._resnet_body(P, img) if self.resnet else self._dla_body_general(P, img)
         # ---- FPN (fpn_patch.py:29-61)
         Cc = self.C
         R = cfg.MODEL.RPN
@@ -1209,43 +1092,17 @@ class Engine(object):
     # ------------------------------------------------------------------------------------------
     # per-frame entry points
     # ------------------------------------------------------------------------------------------
-    def branch_ws(self, b, slot=0):
-        """Split-K scratch of parallel branch b (concurrent convolutions must not share one).  With several backbone streams
-        (clip_backbone_streams > 1) the backbones of consecutive frames run concurrently: one set per plan slot."""
-        key = (slot if self.clip_backbone_streams > 1 else 0, b)
-        if key not in self._branch_ws:
-            self._branch_ws[key] = ops.conv_workspace(self.device)
-        return self._branch_ws[key]
-
-    def backbone_ws(self, slot):
-        """Split-K scratch of the backbone half of plan slot `slot` (shared by all slots while one stream runs them in turn)."""
-        if self.clip_backbone_streams <= 1 or slot == 0:
-            return self.conv_ws
-        if slot not in self._slot_ws:
-            self._slot_ws[slot] = ops.conv_workspace(self.device)
-        return self._slot_ws[slot]
-
-    def backbone_stream(self, t):
-        """The stream the backbone half of clip frame t runs on: frames alternate over clip_backbone_streams low-priority
-        streams, so the (GPU-underfilling, fixed-cost-dominated) layers of consecutive frames' backbones interleave."""
-        n = max(1, self.clip_backbone_streams)
-        if n == 1:
-            return self.side_stream()
-        while len(self._bb_streams) < n:
-            self._bb_streams.append(self.side_stream() if not self._bb_streams else torch.cuda.Stream(device=self.device))
-        return self._bb_streams[t % n]
+    def branch_ws(self, b):
+        """Split-K scratch of parallel branch b (concurrent convolutions must not share one).  Every plan shares it: the
+        backbone halves, which hold the branches, run one after another on one stream."""
+        if b not in self._branch_ws:
+            self._branch_ws[b] = ops.conv_workspace(self.device)
+        return self._branch_ws[b]
 
     def branch_streams(self, n):
         while len(self._branch_streams) < n:
             self._branch_streams.append(torch.cuda.Stream(device=self.device))
         return self._branch_streams[:n]
-
-    def enqueuer(self):
-        """The helper thread of the clip pipeline (started on first use)."""
-        if self._enqueuer is None or not self._enqueuer.is_alive():
-            self._enqueuer = _Enqueuer()
-            self._enqueuer.start()
-        return self._enqueuer
 
     def side_stream(self):
         """The stream forward_clip runs the frame-independent stage on (created on first use)."""
@@ -1271,25 +1128,6 @@ class Engine(object):
         with self.timed("static"):
             P.run() if part is None else P.run_part(part)
         return P
-
-    def static_key(self, frame, slot):
-        """Key of the static plan a clip frame (normalised tensor or decoded uint8 frame) runs on."""
-        if not torch.is_tensor(frame) or frame.dtype == torch.uint8:
-            H, W = self.preprocessor().output_size(frame.shape[0], frame.shape[1])
-        else:
-            H, W = frame.shape[-2], frame.shape[-1]
-        return (H, W, slot)
-
-    def static_ready(self, frame, slot):
-        """True when the frame's static plan exists with both halves captured as CUDA graphs (and, for a decoded frame, its
-        preprocessing buffers exist): replaying it needs no allocation and no capture, so any thread may enqueue it."""
-        P = self.plans.get(self.static_key(frame, slot))
-        if P is None or ((P.part_graphs[0] is None or P.part_graphs[1] is None) and not self.clip_thread_force):
-            return False
-        if not torch.is_tensor(frame) or frame.dtype == torch.uint8:
-            lane = slot if self.clip_backbone_streams > 1 else 0
-            return (frame.shape[0], frame.shape[1], lane) in self.preprocessor()._geo
-        return True
 
     def pair_ok(self, frames):
         """Frame pairs need kernels that take a batch (everything but the DCN gather) and frames of one size and kind."""
@@ -1343,7 +1181,7 @@ class Engine(object):
         oh, ow = pre.output_size(frame.shape[0], frame.shape[1])
         P = self.plan(oh, ow, slot)
         with self.timed("preprocess"):
-            pre.into(frame, P.img_in, slot if self.clip_backbone_streams > 1 else 0)
+            pre.into(frame, P.img_in)
         with self.timed("static"):
             P.run() if part is None else P.run_part(part)
         return P

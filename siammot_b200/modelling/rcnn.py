@@ -10,7 +10,6 @@ through :class:`siammot_b200.engine.Engine`; this file is host control flow only
 TrackHead.get_track_memory track_head.py:54-110), restructured so that a frame costs one
 device->host copy.
 """
-import threading
 import time
 
 import numpy as np
@@ -371,7 +370,7 @@ class CombinedROIHeads(nn.ModuleDict):
             out.append(r)
         return out
 
-    def finish_frame(self, pending, next_P=None, defer=None, before_solver=None):
+    def finish_frame(self, pending, next_P=None, defer=None):
         """Wait for the frame's result block, resolve ids on the host, build the next-frame memory.
         next_P: the static plan the NEXT frame will run on (clip pipelining); defaults to this frame's.
         defer: a list -> the host work nothing downstream waits for (the result BoxList, the per-id cache update) is appended
@@ -383,8 +382,6 @@ class CombinedROIHeads(nn.ModuleDict):
         ht = self.engine.host_timers
         t0 = time.perf_counter() if ht is not None else 0.0
         tp.wait()
-        if before_solver is not None:     # (clip pipeline with a helper thread: the previous frame's cache update must be in)
-            before_solver()
         t1 = time.perf_counter() if ht is not None else 0.0
         # ---- host: unpack the result block
         total, ncap = tp.total, tp.ncap
@@ -799,7 +796,7 @@ def _forward_clip(self, frames, before_frame=None, given_detections=None):
             _run_deferred(deferred, results)       # frame t-1's result object / cache update, under frame t's track stage
             if t + 1 < n_frames:
                 P_next = static(t + 1)
-            result, mem = self.roi_heads.finish_frame(pending, next_P=P_next, defer=deferred if eng.clip_defer else None)
+            result, mem = self.roi_heads.finish_frame(pending, next_P=P_next, defer=deferred)
             ev = torch.cuda.Event()
             ev.record(cur)
             slot_free[t & 1] = ev
@@ -841,21 +838,16 @@ def _forward_clip_three_stage(self, eng, frames, before_frame=None, given_detect
     sD.wait_stream(cur)
     slot_free = [None] * K         # event: every reader of the slot's buffers (D, T, template pooling) is enqueued-complete
     plans = {}
-    extra = []                     # further backbone streams in use (Engine.backbone_stream)
 
     def backbone(t):
         s = t % K
-        sB = eng.backbone_stream(t)           # sA, or one of several alternating backbone streams
-        if sB is not sA and sB not in extra:
-            sB.wait_stream(cur)
-            extra.append(sB)
-        with torch.cuda.stream(sB):
+        with torch.cuda.stream(sA):
             if slot_free[s] is not None:
-                sB.wait_event(slot_free[s])
+                sA.wait_event(slot_free[s])
             P = (eng.run_static_raw(frames[t], s, part=0) if _is_raw_frame(frames[t]) else eng.run_static(frames[t], s, part=0))
             if P.backbone_done is None:
                 P.backbone_done = torch.cuda.Event()
-            P.backbone_done.record(sB)
+            P.backbone_done.record(sA)
         plans[t] = P
 
     def detect(t):
@@ -868,91 +860,31 @@ def _forward_clip_three_stage(self, eng, frames, before_frame=None, given_detect
             P.static_done.record(sD)
 
     deferred = []
-    enq = eng.enqueuer() if eng.clip_thread else None
-    det_ready = {}                 # frame -> threading.Event set once its detect() has been ENQUEUED by the helper thread
-    pending_jobs = []              # threading.Events of helper jobs the caller's thread must not run ahead of
-
-    def threaded(t):
-        """The helper thread takes over once every launch it will issue is a captured CUDA graph (a capture on one thread
-        while another issues CUDA calls would be invalidated) and the staging buffers exist: i.e. after a warm first clip."""
-        if enq is None or not (eng.use_graph or eng.clip_thread_force):
-            return False
-        for tt in (t + 1, t + K - 1):
-            if tt < n_frames and not eng.static_ready(frames[tt], tt % K):
-                return False
-        return True
-
     with torch.no_grad():
         for t in range(min(K - 1, n_frames)):
             backbone(t)
         detect(0)
         for t in range(n_frames):
-            ev = det_ready.pop(t, None)
-            if ev is not None:                     # the helper thread enqueued D(t): wait (host side) until it has
-                ev.wait()
-                enq.check()
             P = plans.pop(t)
             if before_frame is not None:
                 before_frame(t)
             cur.wait_event(P.static_done)          # D(t) complete (hence B(t))
             pending = self.roi_heads.launch_frame(P, self._mem, given_detections[t] if given_detections is not None else None)
-            if threaded(t):
-                # helper thread, in this order: D(t+1) (the caller needs it first), frame t-1's deferred host work (its cache
-                # update must be in before this frame's solver), B(t+K-1)
-                if K == 2 and t + 1 < n_frames:
-                    enq.submit(lambda tt=t + 1: backbone(tt))     # two slots: B(t+1) is this iteration's, and D(t+1) follows it
-                if t + 1 < n_frames:
-                    det_ready[t + 1] = threading.Event()
-                    enq.submit(lambda tt=t + 1: detect(tt), det_ready[t + 1])
-                if deferred:
-                    fns, idx = list(deferred), len(results) - 1
-                    del deferred[:]
-                    done = threading.Event()
-                    pending_jobs.append(done)
-
-                    def late(fns=fns, idx=idx):
-                        with torch.cuda.stream(cur):        # a device-resident result is copied on the caller's stream
-                            for fn in fns:
-                                results[idx] = fn()
-                    enq.submit(late, done)
-                if K > 2 and t + K - 1 < n_frames:
-                    enq.submit(lambda tt=t + K - 1: backbone(tt))
-                nxt = None                          # next frame's plan: known without waiting (slot (t+1) % K)
-                if t + 1 < n_frames:
-                    nxt = eng.plans.get(eng.static_key(frames[t + 1], (t + 1) % K))
-                result, mem = self.roi_heads.finish_frame(pending, next_P=nxt, defer=deferred if eng.clip_defer else None,
-                                                          before_solver=lambda: _join(pending_jobs, enq))
-            else:
-                _run_deferred(deferred, results)   # frame t-1's result object / cache update, under frame t's track stage
-                if t + K - 1 < n_frames:
-                    backbone(t + K - 1)            # slot of frame t-1: its slot_free event was recorded in iteration t-1
-                if t + 1 < n_frames:
-                    detect(t + 1)
-                result, mem = self.roi_heads.finish_frame(pending, next_P=plans.get(t + 1), defer=deferred if eng.clip_defer else None)
+            _run_deferred(deferred, results)       # frame t-1's result object / cache update, under frame t's track stage
+            if t + K - 1 < n_frames:
+                backbone(t + K - 1)                # slot of frame t-1: its slot_free event was recorded in iteration t-1
+            if t + 1 < n_frames:
+                detect(t + 1)
+            result, mem = self.roi_heads.finish_frame(pending, next_P=plans.get(t + 1), defer=deferred)
             ev = torch.cuda.Event()
             ev.record(cur)
             slot_free[t % K] = ev
             self.__dict__["_mem"] = self.__dict__["track_memory"] = mem      # (plain attributes: bypass nn.Module.__setattr__)
             results.append(result)
-        if enq is not None:
-            done = threading.Event()
-            enq.submit(None, done)                 # drain the helper thread
-            done.wait()
-            enq.check()
         _run_deferred(deferred, results)
         cur.wait_stream(sA)
         cur.wait_stream(sD)
-        for sB in extra:
-            cur.wait_stream(sB)
     return results
-
-
-def _join(events, enq):
-    """Wait for the helper-thread jobs the caller must not overtake; surface a helper-thread exception."""
-    for ev in events:
-        ev.wait()
-    del events[:]
-    enq.check()
 
 
 def _forward_clip_pairs(self, eng, frames, before_frame=None, given_detections=None):
@@ -1040,7 +972,7 @@ def _forward_clip_pairs(self, eng, frames, before_frame=None, given_detections=N
                 backbone(u + 1)                    # its buffers held the unit before u (or nothing), whose last reader finished in iteration t-1
             if t + 1 < n_frames:
                 detect(t + 1)
-            result, mem = self.roi_heads.finish_frame(pending, next_P=plans.get(t + 1), defer=deferred if eng.clip_defer else None)
+            result, mem = self.roi_heads.finish_frame(pending, next_P=plans.get(t + 1), defer=deferred)
             if t == t0 + count - 1:                # the unit's buffers are free for their next user
                 ev = torch.cuda.Event()
                 ev.record(cur)

@@ -349,48 +349,3 @@ def test_emulated_frame_overlap_equals_golden(monkeypatch):
     for name in ("emm_amodal_expire_192x320", "emm_3class_192x320"):
         got, fake = _run(name, monkeypatch, env={"SMOT_FRAME_OVERLAP": "1"})
         _compare(load_golden(name)["frames"], got)
-
-
-@pytest.mark.parametrize("slots", ["2", "3"])
-def test_emulated_clip_with_the_helper_thread_equals_golden(slots, monkeypatch):
-    """forward_clip's three-stage pipeline with the backbone / detection-tail enqueues and the deferred host work on the helper
-    thread (Engine.clip_thread; on the GPU it takes over once the launch lists are captured graphs -- here it is forced).  The
-    emulated kernels execute at enqueue time on whichever thread enqueues them, so a missing host-side hand-over (detection tail
-    of frame t before its track stage, cache update of frame t-1 before the solver of frame t) changes the results."""
-    monkeypatch.setenv("SMOT_CLIP_SPLIT", "1")
-    monkeypatch.setenv("SMOT_CLIP_SLOTS", slots)
-    monkeypatch.setenv("SMOT_CLIP_THREAD", "1")
-    monkeypatch.setenv("SMOT_CLIP_PAIRS", "0")          # (the frame-pair variant of the pipeline has no helper-thread mode)
-    cabi_emulator.install(monkeypatch)
-    import threading
-    from siammot_b200.modelling import build_siammot
-    for name in ("emm_256x384", "emm_amodal_expire_192x320"):
-        cfg, sd, clip = scenario_inputs(name)
-        cfg.DTYPE = "float32"
-        model = build_siammot(cfg)
-        model.load_state_dict(sd, strict=False)
-        model.eval()
-        gold = load_golden(name)["frames"]
-        for results_on_host in (True, False):
-            model.results_on_host = results_on_host
-            model.reset_siammot_status()
-            eng = model.engine()
-            frames = [clip[t] for t in range(clip.shape[0])]
-            model.forward_clip(frames[:1])                        # builds the plans of every slot the clip will use? only slot 0:
-            for s in range(int(slots)):                           # ... build the others explicitly (the GPU path warms them up)
-                eng.plan(clip.shape[2], clip.shape[3], s)
-            eng.clip_thread_force = True
-            seen = set()
-            orig = eng.run_tail
-
-            def spy(P, orig=orig):
-                seen.add(threading.current_thread().name)
-                return orig(P)
-            eng.run_tail = spy
-            model.reset_siammot_status()
-            got = model.forward_clip(frames)
-            assert "smot-enqueue" in seen, "the helper thread never enqueued a detection tail: %s" % seen
-            assert len(got) == len(gold)
-            for t, (r, g) in enumerate(zip(got, gold)):
-                assert r is not None and torch.equal(r.get_field("ids"), g["ids"]), (name, t)
-                assert float((r.bbox - g["boxes"]).abs().max()) <= 1e-3 if g["boxes"].numel() else True

@@ -193,23 +193,6 @@ def test_deform_im2col_plus_gemm_matches_torchvision(stride, dtype):
     assert rel_err(got.permute(0, 3, 1, 2).float().cpu(), ref) <= (2e-5 if dtype == torch.float32 else 4e-3)
 
 
-@pytest.mark.parametrize("dtype", ["float32", "float16"])
-def test_body_branches_change_nothing(dtype, monkeypatch):
-    """Same kernels, same operands, one more fork / join per stride-2 tree: bit-identical results (fp32 and fp16)."""
-    from test_e2e_gpu import build_model
-
-    def run(flag):
-        monkeypatch.setenv("SMOT_BODY_BRANCHES", flag)
-        cfg, model, clip = build_model("emm_256x384", dtype)
-        assert model.engine().body_branches == (flag == "1")
-        model.reset_siammot_status()
-        return [model(f.to("cuda"))[0] for f in clip]
-
-    for a, b in zip(run("0"), run("1")):
-        assert torch.equal(a.bbox, b.bbox) and torch.equal(a.get_field("ids"), b.get_field("ids"))
-        assert torch.equal(a.get_field("scores"), b.get_field("scores"))
-
-
 def test_frame_overlap_changes_nothing(monkeypatch):
     from test_e2e_gpu import build_model
 

@@ -77,11 +77,19 @@ DLA_FAMILY = {"DLA-46-C-FPN": (64, 64, 128, 256), "DLA-60-FPN": (128, 256, 512, 
               "DLA-169-FPN": (128, 256, 512, 1024)}
 
 
-@pytest.mark.parametrize("arch", sorted(DLA_FAMILY) + ["DLA-34-FPN", "DLA-60-FPN+DCN", "DLA-102-FPN+DCN"])
+@pytest.mark.parametrize("arch", sorted(DLA_FAMILY) + ["DLA-60-FPN+DCN", "DLA-102-FPN+DCN"])
 def test_dla_family_wiring_matches_oracle(arch, monkeypatch):
     """The general concat-free DlaTree plan (bottleneck blocks, nests up to five deep, residual roots, level-2 nests) against
-    the oracle, which tests/test_oracle_dla_family_cpu.py pins to the reference's own dla.py modules.  DLA-34 through the same
-    general builder must equal its hand-laid (GPU-validated) plan's result too."""
+    the oracle, which tests/test_oracle_dla_family_cpu.py pins to the reference's own dla.py modules."""
+    _check_dla_wiring(arch, monkeypatch)
+
+
+def test_dla34_wiring_matches_oracle(monkeypatch):
+    """DLA-34 (basic blocks, two-level nests), whose GPU execution the e2e parity tests validate, through the same builder."""
+    _check_dla_wiring("DLA-34-FPN", monkeypatch)
+
+
+def _check_dla_wiring(arch, monkeypatch):
     import os
     from helpers import CONFIG_DIR
     from oracle.siammot_oracle import OracleSiamMOT
@@ -99,10 +107,7 @@ def test_dla_family_wiring_matches_oracle(arch, monkeypatch):
     cfg.DTYPE = "float32"
     sd = make_state_dict(cfg, 3)
     eng = build_engine_on_host(cfg, sd, monkeypatch)
-    if arch == "DLA-34-FPN":                       # force the general builder for the validated architecture
-        P = engine_plan_with_general_builder(eng, 64, 96)
-    else:
-        P = eng.plan(64, 96)
+    P = eng.plan(64, 96)
     image = torch.randn(3, 64, 96, generator=torch.Generator().manual_seed(2))
     assert run_backbone(P, image) >= 40
     ref = OracleSiamMOT(cfg, sd).features(image)
@@ -111,21 +116,6 @@ def test_dla_family_wiring_matches_oracle(arch, monkeypatch):
         assert got.shape == want.shape
         err = float((got - want).abs().max() / want.abs().max())
         assert err <= 1e-4, "%s FPN level %d: relative error %g" % (arch, l, err)
-
-
-def engine_plan_with_general_builder(eng, H, W):
-    """plan() with DLA-34 routed through _dla_body_general instead of the hand-laid _tree."""
-    import types
-    orig_tree = eng._tree
-
-    def via_general(self, P, name, x, levels, cin, cout, stride, level_root, out=None, rootbuf=None):
-        assert rootbuf is None
-        return self._tree_general(P, name, x, levels, cin, cout, stride, level_root, False, False, out=out)
-    eng._tree = types.MethodType(via_general, eng)
-    try:
-        return eng.plan(H, W)
-    finally:
-        eng._tree = orig_tree
 
 
 def test_r101_wiring_matches_oracle(monkeypatch):
@@ -147,18 +137,3 @@ def test_r101_wiring_matches_oracle(monkeypatch):
     for l, (got, want) in enumerate(zip(P.feats, OracleSiamMOT(cfg, sd).features(image))):
         err = float((got.permute(0, 3, 1, 2) - want).abs().max() / want.abs().max())
         assert err <= 1e-4, "R-101 FPN level %d: relative error %g" % (l, err)
-
-
-def test_body_branches_plan_has_the_forks_and_the_same_result(monkeypatch):
-    from oracle.siammot_oracle import OracleSiamMOT
-    monkeypatch.setenv("SMOT_BODY_BRANCHES", "1")
-    cfg, sd, clip = scenario_inputs("emm_amodal_expire_192x320")
-    cfg.DTYPE = "float32"
-    eng = build_engine_on_host(cfg, sd, monkeypatch)
-    assert eng.body_branches
-    P = eng.plan(clip[0].shape[1], clip[0].shape[2])
-    forks = [i for i, st in enumerate(P.steps) if st[0] == "fork"]
-    assert len(forks) == 2 + 4                       # FPN laterals, RPN chains + the four stride-2 trees with a project (levels 2..5)
-    assert run_backbone(P, clip[0]) >= 50
-    for got, want in zip(P.feats, OracleSiamMOT(cfg, sd).features(clip[0])):
-        assert float((got.permute(0, 3, 1, 2) - want).abs().max() / want.abs().max()) <= 1e-4

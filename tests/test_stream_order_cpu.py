@@ -66,16 +66,6 @@ def test_three_stage_clip_is_schedule_independent(policy, slots, pairs, monkeypa
     _compare(gold, _run_sim(monkeypatch, policy, "clip", env=env))
 
 
-@pytest.mark.parametrize("slots,streams", [("3", "2"), ("4", "3"), ("4", "2")])
-@pytest.mark.parametrize("policy", POLICIES, ids=str)
-def test_three_stage_clip_with_several_backbone_streams_is_schedule_independent(policy, slots, streams, monkeypatch):
-    """SMOT_CLIP_BACKBONE_STREAMS > 1: the backbone halves of consecutive frames run on alternating streams (per-slot buffers,
-    split-K scratch and preprocessing lanes) -- the results must not depend on how those streams interleave."""
-    gold = load_golden(NAME)["frames"]
-    env = {"SMOT_CLIP_SPLIT": "1", "SMOT_CLIP_SLOTS": slots, "SMOT_CLIP_BACKBONE_STREAMS": streams}
-    _compare(gold, _run_sim(monkeypatch, policy, "clip", env=env))
-
-
 def _differs(gold, got):
     try:
         _compare(gold, got)
@@ -176,16 +166,6 @@ def test_device_resident_results_are_schedule_independent(policy, monkeypatch):
                 assert r.bbox.shape == g["boxes"].shape and torch.equal(r.get_field("ids"), g["ids"]), (mode, t)
                 if g["boxes"].numel():
                     assert float((r.bbox - g["boxes"]).abs().max()) <= 1e-3, (mode, t)
-
-
-@pytest.mark.parametrize("policy", ["lazy", "workers_eager", "default_eager", ("random", 7), ("random", 8)], ids=str)
-def test_body_branches_are_schedule_independent(policy, monkeypatch):
-    """SMOT_BODY_BRANCHES=1: inside the DLA trees the residual path (max-pool -> project) forks off tree1.conv1 and joins before
-    tree1.conv2 -- per-frame calls and the clip pipeline must not depend on how the branch is scheduled."""
-    gold = load_golden(NAME)["frames"]
-    env = {"SMOT_BODY_BRANCHES": "1"}
-    _compare(gold, _run_sim(monkeypatch, policy, "frame", env=env))
-    _compare(gold, _run_sim(monkeypatch, policy, "clip", env=dict(env, SMOT_CLIP_SPLIT="1", SMOT_CLIP_SLOTS="3")))
 
 
 @pytest.mark.parametrize("policy", POLICIES, ids=str)
