@@ -137,7 +137,7 @@ int smot_roi_align_batched(const smot_pyramid* pyr, const long long* image_strid
                            int max_rois, int channels, int res, int sampling_ratio, void* out, int dtype, void* stream);
 
 /* ---- RPN proposal selection (rpn_patch.py:15-60 + upstream select_over_all_levels) -------------
- * Per level: order anchors by objectness (descending, ties -> lower anchor index), take
+ * Per level: order anchors by objectness (descending, ties -> lower anchor index; logits -0 and +0 are equal), take
  * pre_nms_top_n, decode with BoxCoder(1,1,1,1), clip unless amodal, drop boxes smaller than
  * min_size, NMS(nms_thresh) keeping post_nms_top_n; then the fpn_post_nms_top_n best over all levels.
  * head: fp32 [H*W][head_ld], columns [0,A) = objectness logits, [A + 4a + c] = deltas.
@@ -167,7 +167,7 @@ int smot_rpn_select_batched(const smot_rpn_level* levels, const long long* head_
 
 /* ---- sort + NMS (replaces _C.nms and the host-side mask reduction of upstream nms.cu) ----------
  * Rows i < min(n_max, *count) with scores[i*score_stride] > min_score are candidates.  They are
- * ordered by score descending (ties -> lower index), suppressed with IoU(+1) > thresh, and at most
+ * ordered by score descending (ties -> lower index; scores -0 and +0 are equal), suppressed with IoU(+1) > thresh, and at most
  * max_keep survivors are APPENDED at position *out_count (which is then advanced):
  *   out_index[k] = original row, out_boxes[k], out_scores[k], out_tag[k] = tag  (each may be NULL).
  * thresh <= 0 disables suppression (sort only).  n_max <= 4096. */

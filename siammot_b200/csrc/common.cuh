@@ -97,9 +97,10 @@ __device__ __forceinline__ void st4(__half* p, float4 v) {
   *reinterpret_cast<uint2*>(p) = r;
 }
 
-// monotone float -> uint32 key (larger float => larger key); -0 < +0, NaN sorts high
+// monotone float -> uint32 key (larger float => larger key); -0 and +0 get the same key (they compare equal, so the index
+// decides their order), NaN sorts high
 __device__ __forceinline__ uint32_t float_key(float f) {
-  uint32_t u = __float_as_uint(f);
+  uint32_t u = f == 0.f ? 0u : __float_as_uint(f);
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
 

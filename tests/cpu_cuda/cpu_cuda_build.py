@@ -341,3 +341,102 @@ extern "C" void cpu_conv3x3_s2(const void* in, const void* wt, const float* scal
 
 def build_hires():
     return _compile(generate_hires(), OUT_HIRES, ["-I", CUDA_INCLUDE])
+
+
+# ---- proposal selection / NMS (csrc/select_nms.cu) -------------------------------------------------------------------------
+def _split_top_level(text):
+    """Split a launch configuration `grid, block, smem, stream` at the commas outside parentheses."""
+    parts, depth, cur = [], 0, ""
+    for ch in text:
+        depth += ch == "("
+        depth -= ch == ")"
+        if ch == "," and depth == 0:
+            parts.append(cur.strip())
+            cur = ""
+        else:
+            cur += ch
+    return parts + [cur.strip()]
+
+
+def _host_launches(text):
+    """`kernel<<<grid, block, smem, st>>>(args);` -> a synchronous shim launch of the same grid (the host code around the
+    launches -- argument checks, workspace carving, the shared-memory decision -- is the library's own text)."""
+    def sub(m):
+        kern, cfg, args = m.groups()
+        c = _split_top_level(cfg)
+        smem = c[2] if len(c) > 2 else "0"
+        return "cpu_launch_smem(dim3(%s), dim3(%s), (size_t)(%s), [&] { %s(%s); });" % (c[0], c[1], smem, kern, args)
+    out, n = re.subn(r"(\w+(?:<\w+>)?)<<<(.*?)>>>\((.*?)\);", sub, text, flags=re.S)
+    assert n > 0 and "<<<" not in out
+    return out
+
+
+def generate_select(path, mutation=None):
+    """csrc/select_nms.cu from its first constant to its end -- the sort / NMS, RPN, box-decode and scatter kernels AND the
+    extern "C" entry points that size, carve and launch them -- plus float_key / iou_plus1 of csrc/common.cuh, over
+    shim_warp.h.  `mutation` = (old, new[, old2, new2 ...]) textual substitutions applied to select_nms.cu first (each `old`
+    must occur)."""
+    sel = open(os.path.join(CSRC, "select_nms.cu")).read()
+    common = open(os.path.join(CSRC, "common.cuh")).read()
+    if mutation:
+        for old, new in zip(mutation[0::2], mutation[1::2]):
+            assert old in sel, old
+            sel = sel.replace(old, new)
+    body = sel[sel.index("constexpr int SN_THREADS"):]
+    body = body.replace("extern __shared__ __align__(16) unsigned char smem_raw[];", "unsigned char* smem_raw = cpu_dynamic_smem;")
+    body = re.sub(r"(?<!extern )__shared__ ", "static ", body)   # one block runs at a time: a block's statics are its shared memory
+    body = _host_launches(body)
+    assert "__shared__" not in body
+    helpers = (_function_text(common, r"__device__ __forceinline__ uint32_t float_key") +
+               _function_text(common, r"__device__ __forceinline__ float iou_plus1"))
+    parts = ['#include "shim_warp.h"', '#include "smot.h"', r"""
+#include <cstdarg>
+typedef void* cudaStream_t;
+static char cpu_error[512];
+namespace smot {
+void set_error(const char* fmt, ...) {
+  va_list ap;
+  va_start(ap, fmt);
+  std::vsnprintf(cpu_error, sizeof cpu_error, fmt, ap);
+  va_end(ap);
+}
+}  // namespace smot
+extern "C" const char* cpu_last_error() { return cpu_error; }
+static int cpu_launches = 0;
+extern "C" int cpu_launch_count() { return cpu_launches; }
+#define SMOT_CHECK_ARG(cond, ...)   \
+  do {                              \
+    if (!(cond)) {                  \
+      ::smot::set_error(__VA_ARGS__); \
+      return SMOT_ERR_INVALID;      \
+    }                               \
+  } while (0)
+#define SMOT_CHECK_LAUNCH(name) \
+  do {                          \
+  } while (0)
+// the opt-in grant: the largest dynamic shared memory the kernel may be launched with (checked again at every launch)
+#define SMOT_ENSURE_SMEM(kernel, bytes, what)                                                 \
+  do {                                                                                        \
+    if ((size_t)(bytes) > sizeof cpu_dynamic_smem) {                                          \
+      ::smot::set_error("%s: %zu bytes of shared memory", what, (size_t)(bytes));             \
+      return SMOT_ERR_CUDA;                                                                   \
+    }                                                                                         \
+  } while (0)
+static void cpu_launch_smem(dim3 grid, dim3 block, size_t smem, const std::function<void()>& body) {
+  if (smem > sizeof cpu_dynamic_smem) {
+    std::fprintf(stderr, "launch with %zu bytes of dynamic shared memory\n", smem);
+    std::abort();
+  }
+  ++cpu_launches;
+  cpu_launch_warps(grid, block, body);
+}
+namespace smot {""", helpers, body]
+    with open(path, "w") as f:
+        f.write("// GENERATED by tests/cpu_cuda/cpu_cuda_build.py from siammot_b200/csrc/select_nms.cu -- do not edit\n" +
+                "\n".join(parts) + "\n")
+    return path
+
+
+def build_select(out, mutation=None):
+    """Compile generate_select's text into the shared library `out` (its .cpp is written beside it)."""
+    return _compile(generate_select(os.path.splitext(out)[0] + ".cpp", mutation), out, ["-I", os.path.join(REPO, "include")])

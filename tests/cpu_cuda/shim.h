@@ -57,8 +57,8 @@ static inline float __int_as_float(int v) { float f; std::memcpy(&f, &v, 4); ret
 using std::max;
 using std::min;
 
-// dynamic shared memory of the block that is running (blocks are sequential)
-alignas(128) unsigned char cpu_dynamic_smem[160 * 1024];
+// dynamic shared memory of the block that is running (blocks are sequential): the H100 opt-in maximum per block
+alignas(128) unsigned char cpu_dynamic_smem[227 * 1024];
 
 namespace smot {
 // csrc/common.cuh, host restatement of what the simple kernels use

@@ -10,24 +10,13 @@
 // xcorr_mma_kernel -- validated on the GPU -- runs through the same emulation, which is what validates the emulation.
 #pragma once
 #define SHIM_WITH_CUDA_FP16
-#include "shim.h"
+#include "shim_warp.h"
 
-#include <atomic>
 #include <cstdlib>
 
 static inline uint32_t cpu_smem_offset(const void* p) { return (uint32_t)((const unsigned char*)p - cpu_dynamic_smem); }
 #define __cvta_generic_to_shared(p) ((size_t)cpu_smem_offset(p))
 static inline void __trap() { std::abort(); }
-
-constexpr int CPU_MAX_WARPS = 32;
-struct CpuWarp {
-  std::barrier<>* bar = nullptr;
-  uint32_t addr[32];
-  uint32_t a[32][4], b[32][2];
-};
-static CpuWarp cpu_warps[CPU_MAX_WARPS];
-static inline CpuWarp& cpu_my_warp() { return cpu_warps[threadIdx.x >> 5]; }
-static inline void __syncwarp() { cpu_my_warp().bar->arrive_and_wait(); }
 
 static inline float cpu_h2f(uint32_t word, int hi) {
   __half h;
@@ -116,15 +105,3 @@ inline void xp_bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t 
 }
 
 }  // namespace smot
-
-// cpu_launch for kernels with warp collectives: per-warp barriers for the block that is running
-static inline void cpu_launch_warps(dim3 grid, dim3 block, const std::function<void()>& body) {
-  const unsigned nwarps = block.x / 32;
-  std::vector<std::barrier<>*> bars;
-  for (unsigned i = 0; i < nwarps; ++i) {
-    bars.push_back(new std::barrier<>(32));
-    cpu_warps[i].bar = bars.back();
-  }
-  cpu_launch(grid, block, body);
-  for (auto* b : bars) delete b;
-}
