@@ -441,7 +441,9 @@ __global__ void __launch_bounds__(TC_THREADS, STAGES == 2 ? 2 : 1) conv_tc_kerne
     }
     if (threadIdx.x == 0) TC_STAMP(4);
   }
-  if constexpr (STAGES > 2)   // the 2-stage variants run 2 CTAs per SM on full-GPU layers: they never split K, keep their registers low
+  // the 2-stage variants run 2 CTAs per SM and keep their registers low: they carry no cluster finish, and conv2d_tc never
+  // launches them with cluster_reduce set (when they split K, their partials go to splitk_reduce_kernel)
+  if constexpr (STAGES > 2)
   if (a.cluster_reduce) {
     // every CTA of the tile's cluster has parked its partial: publish (gpu scope), meet, finish 128 / splits rows each
     __threadfence();
@@ -744,6 +746,20 @@ static int tc_stages(int BN, bool solo, bool shallow, int my_chunks, int forced)
   return deep ? 8 : (shallow ? 2 : 4);
 }
 
+// ring depth of a launch of `ctas` CTAs over `tiles_n` = tiles x N tiles, `my_chunks` K chunks per CTA (or per slice owner).
+// `finish`: the CTA finishes the tile itself (in-CTA K slices or the cluster finish), which the 2-stage variants carry no
+// code for: lift them to the 3 / 4-stage ring of the same N tile.
+static int tc_launch_stages(int BN, long long ctas, long long tiles_n, int all_chunks, int my_chunks, int forced, bool finish) {
+  // many short tiles: 2-stage rings let 2 CTAs share an SM, so one CTA's prologue / epilogue overlaps the
+  // main loops of the others (the same bytes in flight per SM as one CTA with 4 stages)
+  const bool shallow = forced ? forced == 2 : (tiles_n >= 296 && all_chunks <= 36);
+  // at most one CTA per SM: nothing else hides the TMA round trip (the loop then advances `ring depth` chunks
+  // per round trip), so use the whole shared memory for the ring: 8 x 24 KB, 6 x 32 KB, 4 x 48 KB
+  const bool solo = ctas <= sm_count();
+  const int stages = tc_stages(BN, solo, shallow, my_chunks, forced);
+  return (finish && stages == 2) ? (BN == 128 ? 3 : 4) : stages;
+}
+
 #define SMOT_TC_DISPATCH(BN_, ST_, EXPR)                                                       \
   ((BN_) == 256 ? ((ST_) == 4 ? EXPR(256, 4) : EXPR(256, 3))                                    \
    : (BN_) == 128 ? ((ST_) == 2 ? EXPR(128, 2) : ((ST_) == 6 ? EXPR(128, 6) : EXPR(128, 3)))   \
@@ -874,7 +890,9 @@ int conv2d_tc(const smot_conv_desc* d, cudaStream_t st) {
           const int cps = (all_chunks + cz - 1) / cz;
           const int real = (all_chunks + cps - 1) / cps;                       // no empty split
           if (real != cz) continue;
-          const int stg = tc_stages(bw, true, false, cps, fs);
+          // the occupancy of the variant this cluster launch would run (never a 2-stage one: they carry no finish)
+          const long long tiles_n = tiles * (d->Cout / bw);
+          const int stg = tc_launch_stages(bw, tiles_n * cz, tiles_n, all_chunks, cps, fs, true);
 #define SMOT_TC_MAXC(BN_, ST_) tc_max_clusters<BN_, ST_>(cz)
           const int fit = SMOT_TC_DISPATCH(bw, stg, SMOT_TC_MAXC);
 #undef SMOT_TC_MAXC
@@ -933,14 +951,8 @@ int conv2d_tc(const smot_conv_desc* d, cudaStream_t st) {
   }
   a.partial = d->workspace ? (float*)((char*)d->workspace + SMOT_CONV_WS_COUNTER_BYTES) : nullptr;
   dim3 grid((unsigned)tiles, (unsigned)(d->Cout / BN), (unsigned)a.splits);
-  // many short tiles: 2-stage rings let 2 CTAs share an SM, so one CTA's prologue / epilogue overlaps the
-  // main loops of the others (the same bytes in flight per SM as one CTA with 4 stages)
-  const bool shallow = fs ? fs == 2 : (tiles * (d->Cout / BN) >= 296 && all_chunks <= 36);
-  // at most one CTA per SM: nothing else hides the TMA round trip (the loop then advances `ring depth` chunks
-  // per round trip), so use the whole shared memory for the ring: 8 x 24 KB, 6 x 32 KB, 4 x 48 KB
-  const bool solo = (long long)grid.x * grid.y * grid.z <= sm_count();
-  int stages = tc_stages(BN, solo, shallow, sliced ? all_chunks : a.chunks_per_split, fs);
-  if (sliced && stages == 2) stages = BN == 128 ? 3 : 4;   // the 2-stage variants carry no slice code
+  const int stages = tc_launch_stages(BN, (long long)grid.x * grid.y * grid.z, tiles * (d->Cout / BN), all_chunks,
+                                      sliced ? all_chunks : a.chunks_per_split, fs, sliced || a.cluster_reduce);
 #define SMOT_TC_LAUNCH(BN_, ST_) launch_tc<BN_, ST_>(tmA, tmB, a, grid, st)
   const int rc = SMOT_TC_DISPATCH(BN, stages, SMOT_TC_LAUNCH);
 #undef SMOT_TC_LAUNCH

@@ -3,7 +3,8 @@
 Tolerances: SMOT_F32 kernels use IEEE fp32 multiply-adds, so they agree with the CPU oracle up to
 summation order: 2e-5 relative to the output scale.  SMOT_F16 (fp16 storage, fp32 accumulate) is
 compared with the oracle evaluated on the fp16-rounded inputs: 2e-3 relative (output rounding).
-Integer / index outputs (NMS keep lists, arg-max, levels, counts) must be bit-exact.
+Integer / index outputs (NMS keep lists, arg-max, levels, counts) must be bit-exact.  Convolutions are checked element by
+element against the float64 reference and bound of tests/launch_check.py (conv2d_checked).
 """
 import math
 
@@ -44,6 +45,23 @@ def tol(dtype):
     return 2e-5 if dtype == torch.float32 else 2e-3
 
 
+def conv2d_checked(x, weight, scale=None, bias=None, residual=None, stride=1, pad=0, relu=False, out=None, out_dtype=None,
+                   algo=0, workspace=None):
+    """ops.conv2d, its output checked element by element against the float64 reference and bound of
+    tests/launch_check.py (check_conv)."""
+    import launch_check as lc
+    B, H, W, _ = x.shape
+    KH, KW = weight.shape[1], weight.shape[2]
+    if out is None:
+        out = torch.empty((B, (H + 2 * pad - KH) // stride + 1, (W + 2 * pad - KW) // stride + 1, weight.shape[0]),
+                          dtype=out_dtype or x.dtype, device=x.device)
+    d = ops().conv_desc(x, weight, out, scale, bias, residual, stride, pad, relu, algo, workspace)
+    ck = lc.check_conv(lc.Memory(DEV), d, lambda: ops().conv2d(x, weight, scale, bias, residual, stride, pad, relu, out=out,
+                                                               algo=algo, workspace=workspace))
+    assert ck.max_ratio <= 1.0, "conv %s: |err|/bound %.3f at %s" % (lc.describe_conv(d), ck.max_ratio, ck.where)
+    return out
+
+
 def q(x, dtype):
     """Round through the storage dtype (so the oracle sees the same inputs)."""
     return x.to(dtype).float()
@@ -74,20 +92,11 @@ def test_conv2d(case, dtype):
     bias = torch.randn(Cout, generator=g)
     OH, OW = (H + 2 * pad - k) // stride + 1, (W + 2 * pad - k) // stride + 1
     res = q(torch.randn(B, Cout, OH, OW, generator=g), dtype) if use_res else None
-    ref = F.conv2d(x, w, None, stride, pad)
-    if scale is not None:
-        ref = ref * scale.view(1, -1, 1, 1)
-    ref = ref + bias.view(1, -1, 1, 1)
-    if res is not None:
-        ref = ref + res
-    if relu:
-        ref = F.relu(ref)
     out_dtype = torch.float32 if Cout == 15 else dtype
-    got = ops().conv2d(nhwc(x, dtype), ohwi(w, dtype), scale.to(DEV) if scale is not None else None, bias.to(DEV),
-                       nhwc(res, dtype) if res is not None else None, stride, pad, relu, out_dtype=out_dtype)
+    got = conv2d_checked(nhwc(x, dtype), ohwi(w, dtype), scale.to(DEV) if scale is not None else None, bias.to(DEV),
+                         nhwc(res, dtype) if res is not None else None, stride, pad, relu, out_dtype=out_dtype)
     torch.cuda.synchronize()
     assert got.dtype == out_dtype
-    assert rel_err(nchw(got), ref) <= (tol(dtype) if out_dtype == dtype else tol(dtype))
 
 
 @pytest.mark.parametrize("dtype", [torch.float32, torch.float16])
@@ -99,30 +108,24 @@ def test_conv2d_concat_free_root_and_fc(dtype):
     parts = [q(torch.randn(1, c, H, W, generator=g), dtype) for c in (64, 64, 32)]
     w = q(torch.randn(48, 160, 1, 1, generator=g) / math.sqrt(160), dtype)
     scale, bias = 0.5 + torch.rand(48, generator=g), torch.randn(48, generator=g)
-    ref = F.relu(F.conv2d(torch.cat(parts, 1), w) * scale.view(1, -1, 1, 1) + bias.view(1, -1, 1, 1))
     buf = torch.zeros(1, H, W, 160, dtype=dtype, device=DEV)
     off = 0
     for p in parts:
         buf[..., off:off + p.shape[1]] = nhwc(p, dtype)
         off += p.shape[1]
     outbuf = torch.zeros(1, H, W, 112, dtype=dtype, device=DEV)
-    ops().conv2d(buf, ohwi(w, dtype), scale.to(DEV), bias.to(DEV), relu=True, out=outbuf[..., 64:112])
+    conv2d_checked(buf, ohwi(w, dtype), scale.to(DEV), bias.to(DEV), relu=True, out=outbuf[..., 64:112])
     torch.cuda.synchronize()
-    assert rel_err(nchw(outbuf[..., 64:112]), ref) <= tol(dtype)
     assert float(outbuf[..., :64].abs().max()) == 0.0
     # a 3x3 conv whose INPUT is a slice (pitch 160) of the buffer
     w3 = q(torch.randn(64, 64, 3, 3, generator=g) / 24.0, dtype)
-    ref3 = F.conv2d(parts[1], w3, None, 1, 1)
-    got3 = ops().conv2d(buf[..., 64:128], ohwi(w3, dtype), pad=1)
-    assert rel_err(nchw(got3), ref3) <= tol(dtype)
+    conv2d_checked(buf[..., 64:128], ohwi(w3, dtype), pad=1)
     # fully connected: 77 rows x 6272 -> 1024 (box head fc6 shape)
     xfc = q(torch.randn(77, 6272, generator=g), dtype)
     wfc = q(torch.randn(1024, 6272, generator=g) / math.sqrt(6272), dtype)
     bfc = torch.randn(1024, generator=g)
-    reffc = F.relu(F.linear(xfc, wfc, bfc))
-    gotfc = ops().conv2d(xfc.to(DEV, dtype).view(1, 1, 77, 6272), wfc.to(DEV, dtype).view(1024, 1, 1, 6272), None,
-                         bfc.to(DEV), relu=True)
-    assert rel_err(gotfc.view(77, 1024).float().cpu(), reffc) <= tol(dtype)
+    conv2d_checked(xfc.to(DEV, dtype).view(1, 1, 77, 6272), wfc.to(DEV, dtype).view(1024, 1, 1, 6272), None,
+                   bfc.to(DEV), relu=True)
 
 
 @pytest.mark.parametrize("dtype", [torch.float32, torch.float16])
@@ -347,8 +350,8 @@ TC_CASES = [
 
 @pytest.mark.parametrize("case", TC_CASES)
 def test_conv2d_tcgen05_matches_oracle_and_simt(case):
-    """The wgmma/TMA member of the conv family against torch fp32 on the fp16-rounded operands and
-    against the SIMT member (same operands, fp32 accumulation in both)."""
+    """The wgmma/TMA member of the conv family and the SIMT member on the same fp16 operands, each within the float64
+    bound of tests/launch_check.py."""
     from siammot_b200 import _lib
     B, Cin, H, W, Cout, k, use_res, relu, use_scale = case
     g = torch.Generator().manual_seed(Cin + H)
@@ -358,24 +361,14 @@ def test_conv2d_tcgen05_matches_oracle_and_simt(case):
     scale = (0.5 + torch.rand(Cout, generator=g)) if use_scale else None
     bias = torch.randn(Cout, generator=g)
     res = q(torch.randn(B, Cout, H, W, generator=g), dt) if use_res else None
-    ref = F.conv2d(x, w, None, 1, k // 2)
-    if scale is not None:
-        ref = ref * scale.view(1, -1, 1, 1)
-    ref = ref + bias.view(1, -1, 1, 1)
-    if res is not None:
-        ref = ref + res
-    if relu:
-        ref = F.relu(ref)
     dx, dw = nhwc(x, dt), ohwi(w, dt)
     ds, db = (scale.to(DEV) if scale is not None else None), bias.to(DEV)
     dr = nhwc(res, dt) if res is not None else None
     out = torch.empty((B, H, W, Cout), dtype=dt, device=DEV)
     assert ops().conv2d_algo(dx, dw, out, scale=ds, bias=db, residual=dr, pad=k // 2, relu=relu) == _lib.CONV_TCGEN05
-    got_tc = ops().conv2d(dx, dw, ds, db, dr, 1, k // 2, relu, algo=_lib.CONV_TCGEN05)
-    got_simt = ops().conv2d(dx, dw, ds, db, dr, 1, k // 2, relu, algo=_lib.CONV_SIMT)
+    conv2d_checked(dx, dw, ds, db, dr, 1, k // 2, relu, algo=_lib.CONV_TCGEN05)
+    conv2d_checked(dx, dw, ds, db, dr, 1, k // 2, relu, algo=_lib.CONV_SIMT)
     torch.cuda.synchronize()
-    assert rel_err(nchw(got_tc), ref) <= 2e-3
-    assert rel_err(nchw(got_tc), nchw(got_simt)) <= 1e-3
 
 
 def test_conv2d_tcgen05_channel_slices_and_fc():
@@ -388,20 +381,16 @@ def test_conv2d_tcgen05_channel_slices_and_fc():
     outbuf = torch.zeros(1, H, W, 192, dtype=dt, device=DEV)
     x_view, o_view = buf[..., 64:192], outbuf[..., 128:192]
     res_view = buf[..., 256:320]
-    ref = F.relu(F.conv2d(nchw(x_view), w3, None, 1, 1) + nchw(res_view))
     assert ops().conv2d_algo(x_view, ohwi(w3, dt), o_view, residual=res_view, pad=1, relu=True) == _lib.CONV_TCGEN05
-    ops().conv2d(x_view, ohwi(w3, dt), residual=res_view, pad=1, relu=True, out=o_view)
+    conv2d_checked(x_view, ohwi(w3, dt), residual=res_view, pad=1, relu=True, out=o_view)
     torch.cuda.synchronize()
-    assert rel_err(nchw(o_view), ref) <= 2e-3
     assert float(outbuf[..., :128].abs().max()) == 0.0
     for rows in (300, 30, 128):
         xfc = q(torch.randn(rows, 6272, generator=g), dt)
         wfc = q(torch.randn(1024, 6272, generator=g) / math.sqrt(6272), dt)
         bfc = torch.randn(1024, generator=g)
-        reffc = F.relu(F.linear(xfc, wfc, bfc))
-        gotfc = ops().conv2d(xfc.to(DEV, dt).view(1, 1, rows, 6272), wfc.to(DEV, dt).view(1024, 1, 1, 6272), None,
-                             bfc.to(DEV), relu=True, algo=_lib.CONV_TCGEN05)
-        assert rel_err(gotfc.view(rows, 1024).float().cpu(), reffc) <= 2e-3
+        conv2d_checked(xfc.to(DEV, dt).view(1, 1, rows, 6272), wfc.to(DEV, dt).view(1024, 1, 1, 6272), None,
+                       bfc.to(DEV), relu=True, algo=_lib.CONV_TCGEN05)
 
 
 @pytest.mark.parametrize("case", [(1, 64, 88, 160, 128), (1, 128, 44, 80, 256), (1, 256, 22, 40, 512), (2, 64, 32, 48, 64)])
@@ -414,15 +403,12 @@ def test_conv2d_tcgen05_stride2(case):
     x = q(torch.randn(B, Cin, H, W, generator=g), dt)
     w = q(torch.randn(Cout, Cin, 3, 3, generator=g) / math.sqrt(Cin * 9), dt)
     scale, bias = 0.5 + torch.rand(Cout, generator=g), torch.randn(Cout, generator=g)
-    ref = F.relu(F.conv2d(x, w, None, 2, 1) * scale.view(1, -1, 1, 1) + bias.view(1, -1, 1, 1))
     out = torch.empty((B, H // 2, W // 2, Cout), dtype=dt, device=DEV)
     args = (nhwc(x, dt), ohwi(w, dt), scale.to(DEV), bias.to(DEV), None, 2, 1, True)
     assert ops().conv2d_algo(args[0], args[1], out, scale=args[2], bias=args[3], stride=2, pad=1, relu=True) == _lib.CONV_TCGEN05
-    got = ops().conv2d(*args, algo=_lib.CONV_TCGEN05)
-    got_simt = ops().conv2d(*args, algo=_lib.CONV_SIMT)
+    conv2d_checked(*args, algo=_lib.CONV_TCGEN05)
+    conv2d_checked(*args, algo=_lib.CONV_SIMT)
     torch.cuda.synchronize()
-    assert rel_err(nchw(got), ref) <= 2e-3
-    assert rel_err(nchw(got), nchw(got_simt)) <= 1e-3
 
 
 @pytest.mark.parametrize("dtype", [torch.float32, torch.float16])
@@ -436,19 +422,15 @@ def test_conv2d_small_cout_kernel(dtype):
     for (lo, hi, cout, off, relu) in ((0, 128, 3, 0, False), (128, 256, 4, 3, True)):
         w = q(torch.randn(cout, 128, 3, 3, generator=g) / 34.0, dtype)
         b = torch.randn(cout, generator=g)
-        ref = F.conv2d(tower[:, lo:hi], w, b, 1, 1)
-        ref = F.relu(ref) if relu else ref
-        ops().conv2d(dtower[..., lo:hi], ohwi(w, dtype), None, b.to(DEV), pad=1, relu=relu, out=maps[..., off:off + cout])
-        assert rel_err(nchw(maps[..., off:off + cout]), ref) <= tol(dtype)
+        conv2d_checked(dtower[..., lo:hi], ohwi(w, dtype), None, b.to(DEV), pad=1, relu=relu, out=maps[..., off:off + cout])
     assert float(maps[..., 7].abs().max()) == 0.0
     for rows in (300, 30, 1):
         x = q(torch.randn(rows, 1024, generator=g), dtype)
         w = q(torch.randn(10, 1024, generator=g) / 32.0, dtype)
         b = torch.randn(10, generator=g)
         out = torch.zeros(1, 1, rows, 12, dtype=torch.float32, device=DEV)
-        ops().conv2d(x.to(DEV, dtype).view(1, 1, rows, 1024), w.to(DEV, dtype).view(10, 1, 1, 1024), None, b.to(DEV),
-                     out=out[..., :10])
-        assert rel_err(out[0, 0, :, :10].cpu(), F.linear(x, w, b)) <= tol(dtype)
+        conv2d_checked(x.to(DEV, dtype).view(1, 1, rows, 1024), w.to(DEV, dtype).view(10, 1, 1, 1024), None, b.to(DEV),
+                       out=out[..., :10])
         assert float(out[..., 10:].abs().max()) == 0.0
     # RPN predictor: 1x1, 128 -> 15 (objectness + deltas), fp32 head with pitch 16; ragged pixel counts, batch 2
     for (B, H, W) in ((1, 22, 40), (1, 11, 20), (2, 5, 7), (1, 44, 80)):
@@ -456,16 +438,13 @@ def test_conv2d_small_cout_kernel(dtype):
         w = q(torch.randn(15, 128, 1, 1, generator=g) / 11.0, dtype)
         b = torch.randn(15, generator=g)
         head = torch.zeros(B, H, W, 16, dtype=torch.float32, device=DEV)
-        ops().conv2d(nhwc(x, dtype), ohwi(w, dtype), None, b.to(DEV), out=head[..., :15])
-        assert rel_err(nchw(head[..., :15]), F.conv2d(x, w, b)) <= tol(dtype)
+        conv2d_checked(nhwc(x, dtype), ohwi(w, dtype), None, b.to(DEV), out=head[..., :15])
         assert float(head[..., 15].abs().max()) == 0.0
     # fp16 output with scale + bias + ReLU (the generic epilogue)
     x = q(torch.randn(2, 64, 9, 13, generator=g), dtype)
     w = q(torch.randn(8, 64, 3, 3, generator=g) / 24.0, dtype)
     sc, b = torch.rand(8, generator=g) + 0.5, torch.randn(8, generator=g)
-    ref = F.relu(F.conv2d(x, w, None, 1, 1) * sc[None, :, None, None] + b[None, :, None, None])
-    got = ops().conv2d(nhwc(x, dtype), ohwi(w, dtype), sc.to(DEV), b.to(DEV), pad=1, relu=True)
-    assert rel_err(nchw(got), ref) <= tol(dtype)
+    conv2d_checked(nhwc(x, dtype), ohwi(w, dtype), sc.to(DEV), b.to(DEV), pad=1, relu=True)
 
 
 HIRES_CASES = [
@@ -480,7 +459,7 @@ HIRES_CASES = [
 
 @pytest.mark.parametrize("case", HIRES_CASES)
 def test_conv2d_hires_kernels(case):
-    """mma.sync halo-tile kernels of the DLA stem / levels 0-1 (fp16): vs torch fp32 and vs the SIMT kernel."""
+    """mma.sync halo-tile kernels of the DLA stem / levels 0-1 (fp16) and the SIMT kernel, each within the float64 bound."""
     from siammot_b200 import _lib
     name, Cin, Cout, k, stride, H, W = case
     g = torch.Generator().manual_seed(len(name) + H)
@@ -488,7 +467,6 @@ def test_conv2d_hires_kernels(case):
     x = q(torch.randn(2, Cin, H, W, generator=g), dt)
     w = q(torch.randn(Cout, Cin, k, k, generator=g) / math.sqrt(Cin * k * k), dt)
     scale, bias = 0.5 + torch.rand(Cout, generator=g), torch.randn(Cout, generator=g)
-    ref = F.relu(F.conv2d(x, w, None, stride, k // 2) * scale.view(1, -1, 1, 1) + bias.view(1, -1, 1, 1))
     if Cin == 3:
         buf = torch.zeros(2, H, W, 4, dtype=dt, device=DEV)
         buf[..., :3] = nhwc(x, dt)
@@ -496,11 +474,9 @@ def test_conv2d_hires_kernels(case):
     else:
         dx = nhwc(x, dt)
     args = (dx, ohwi(w, dt), scale.to(DEV), bias.to(DEV), None, stride, k // 2, True)
-    got = ops().conv2d(*args)                       # AUTO -> hires kernel
-    got_simt = ops().conv2d(*args, algo=_lib.CONV_SIMT)
+    conv2d_checked(*args)                       # AUTO -> hires kernel
+    conv2d_checked(*args, algo=_lib.CONV_SIMT)
     torch.cuda.synchronize()
-    assert rel_err(nchw(got), ref) <= 2e-3
-    assert rel_err(nchw(got), nchw(got_simt)) <= 1e-3
 
 
 @pytest.mark.parametrize("case", [("stem", 3, 16, 7, 1, 2, 704, 1280), ("level0", 16, 16, 3, 1, 1, 352, 640), ("stem", 3, 16, 7, 1, 1, 100, 70),
@@ -517,7 +493,6 @@ def test_conv2d_hires_persistent_kernels(case, monkeypatch):
     x = q(torch.randn(batch, Cin, H, W, generator=g), dt)
     w = q(torch.randn(Cout, Cin, k, k, generator=g) / math.sqrt(Cin * k * k), dt)
     scale, bias = 0.5 + torch.rand(Cout, generator=g), torch.randn(Cout, generator=g)
-    ref = F.relu(F.conv2d(x, w, None, stride, k // 2) * scale.view(1, -1, 1, 1) + bias.view(1, -1, 1, 1))
     if Cin == 3:
         buf = torch.zeros(batch, H, W, 4, dtype=dt, device=DEV)
         buf[..., :3] = nhwc(x, dt)
@@ -526,15 +501,14 @@ def test_conv2d_hires_persistent_kernels(case, monkeypatch):
         dx = nhwc(x, dt)
     args = (dx, ohwi(w, dt), scale.to(DEV), bias.to(DEV), None, stride, k // 2, True)
     monkeypatch.setenv("SMOT_HIRES_PERSIST", "0")
-    per_tile = ops().conv2d(*args)
+    per_tile = conv2d_checked(*args)
     monkeypatch.setenv("SMOT_HIRES_PERSIST", "2")
     for _ in range(2):                               # back-to-back launches chain through PDL
         got = ops().conv2d(*args)
     torch.cuda.synchronize()
     assert torch.equal(got, per_tile)
-    assert rel_err(nchw(got), ref) <= 2e-3
     monkeypatch.delenv("SMOT_HIRES_PERSIST")
-    assert torch.equal(ops().conv2d(*args), per_tile)   # the default rule, whichever kernel it picks
+    assert torch.equal(conv2d_checked(*args), per_tile)   # the default rule, whichever kernel it picks
 
 
 @pytest.mark.parametrize("mode", ["16", "10"])
@@ -552,10 +526,8 @@ def test_conv2d_tcgen05_halo_variant(mode, monkeypatch):
         w = q(torch.randn(Cout, Cin, 3, 3, generator=g) / math.sqrt(Cin * 9), dt)
         res = q(torch.randn(B, Cout, H, W, generator=g), dt)
         scale, bias = 0.5 + torch.rand(Cout, generator=g), torch.randn(Cout, generator=g)
-        ref = F.relu(F.conv2d(x, w, None, 1, 1) * scale.view(1, -1, 1, 1) + bias.view(1, -1, 1, 1) + res)
-        got = ops().conv2d(nhwc(x, dt), ohwi(w, dt), scale.to(DEV), bias.to(DEV), nhwc(res, dt), 1, 1, True,
-                           algo=_lib.CONV_TCGEN05, workspace=ws if use_ws else None)
-        assert rel_err(nchw(got), ref) <= 2e-3
+        conv2d_checked(nhwc(x, dt), ohwi(w, dt), scale.to(DEV), bias.to(DEV), nhwc(res, dt), 1, 1, True,
+                       algo=_lib.CONV_TCGEN05, workspace=ws if use_ws else None)
 
 
 def test_conv2d_tcgen05_split_k():
@@ -570,23 +542,18 @@ def test_conv2d_tcgen05_split_k():
     w = q(torch.randn(512, 512, 3, 3, generator=g) / math.sqrt(512 * 9), dt)
     res = q(torch.randn(1, 512, 22, 40, generator=g), dt)
     scale, bias = 0.5 + torch.rand(512, generator=g), torch.randn(512, generator=g)
-    ref = F.relu(F.conv2d(x, w, None, 1, 1) * scale.view(1, -1, 1, 1) + bias.view(1, -1, 1, 1) + res)
     args = (nhwc(x, dt), ohwi(w, dt), scale.to(DEV), bias.to(DEV), nhwc(res, dt), 1, 1, True)
     for _ in range(2):
-        got = ops().conv2d(*args, algo=_lib.CONV_TCGEN05, workspace=ws)
+        conv2d_checked(*args, algo=_lib.CONV_TCGEN05, workspace=ws)
         torch.cuda.synchronize()
-        assert rel_err(nchw(got), ref) <= 2e-3
-    plain = ops().conv2d(*args, algo=_lib.CONV_TCGEN05)
-    assert rel_err(nchw(got), nchw(plain)) <= 1e-3
+    conv2d_checked(*args, algo=_lib.CONV_TCGEN05)
     # fc6 for 300 and 30 rows
     for rows in (300, 30):
         xfc = q(torch.randn(rows, 6272, generator=g), dt)
         wfc = q(torch.randn(1024, 6272, generator=g) / math.sqrt(6272), dt)
         bfc = torch.randn(1024, generator=g)
-        reffc = F.relu(F.linear(xfc, wfc, bfc))
-        gotfc = ops().conv2d(xfc.to(DEV, dt).view(1, 1, rows, 6272), wfc.to(DEV, dt).view(1024, 1, 1, 6272), None,
-                             bfc.to(DEV), relu=True, algo=_lib.CONV_TCGEN05, workspace=ws)
-        assert rel_err(gotfc.view(rows, 1024).float().cpu(), reffc) <= 2e-3
+        conv2d_checked(xfc.to(DEV, dt).view(1, 1, rows, 6272), wfc.to(DEV, dt).view(1024, 1, 1, 6272), None,
+                       bfc.to(DEV), relu=True, algo=_lib.CONV_TCGEN05, workspace=ws)
     torch.cuda.synchronize()
     assert int(ws[:_lib.CONV_WS_COUNTER_BYTES].view(torch.int32).abs().sum()) == 0
 
@@ -606,14 +573,12 @@ def test_conv2d_tcgen05_k_slices_equal_split_k(case, monkeypatch):
     w = q(torch.randn(Cout, Cin, k, k, generator=g) / math.sqrt(Cin * k * k), dt)
     res = q(torch.randn(B, Cout, H, W, generator=g), dt)
     scale, bias = 0.5 + torch.rand(Cout, generator=g), torch.randn(Cout, generator=g)
-    ref = F.relu(F.conv2d(x, w, None, 1, k // 2) * scale.view(1, -1, 1, 1) + bias.view(1, -1, 1, 1) + res)
     args = (nhwc(x, dt), ohwi(w, dt), scale.to(DEV), bias.to(DEV), nhwc(res, dt), 1, k // 2, True)
     monkeypatch.setenv("SMOT_TC_SLICED", "0")
-    split = ops().conv2d(*args, algo=_lib.CONV_TCGEN05, workspace=ws)
+    split = conv2d_checked(*args, algo=_lib.CONV_TCGEN05, workspace=ws)
     torch.cuda.synchronize()
     monkeypatch.setenv("SMOT_TC_SLICED", "1")
     for _ in range(2):
-        sliced = ops().conv2d(*args, algo=_lib.CONV_TCGEN05, workspace=ws)
+        sliced = conv2d_checked(*args, algo=_lib.CONV_TCGEN05, workspace=ws)
     torch.cuda.synchronize()
-    assert rel_err(nchw(sliced), ref) <= 2e-3
     assert torch.equal(sliced, split)
